@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- hot-path throughput of the spatial-parallel conv engine on B200.
+"""bench.py -- hot-path throughput of the spatial-parallel conv engine on H100.
 
 One "step" = one pass of the hot path over one synthetic image: forward and backward (dgrad +
 wgrad) of every conv / pool layer of the reference's SPATIAL STAGE of AmoebaNet-D(18,416) at
@@ -10,6 +10,7 @@ torchgems.spatial modules (which call libspconv.so through the C ABI).
 
     python bench.py --gpus N --steps K --warmup W            # our arm
     python bench.py --impl reference ...                     # the reference's CPU path (port)
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's outputs as .npy
 
 Prints ONE JSON line (see the task contract): metric/value/unit, ms_per_step, e2e, roofline,
 cpu_baseline, clocks, gpu_launches.
@@ -64,7 +65,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d["hbm_gbs"], d.get("bf16_tflops_sustained", d["bf16_tflops"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1400.0, "fallback (B200_PROFILING.md)"
+    # NVIDIA's H100 SXM data sheet: 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 (at 700 W; not reached in practice)
+    return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -221,7 +223,7 @@ def run_reference(args):
 # ------------------------------------------------------------------------------------------------
 def cudnn_baseline(torch, layers_unique, order, dev, steps, warmup, full_size_cudnn=False):
     """The competitor BASELINE.md section 4 names: the identical layer list on STOCK PyTorch ops on the
-    same B200 -- F.pad (the reference's ZeroPad2d copy, spatial.py:1020 / :1099, on every conv_spatial and
+    same GPU -- F.pad (the reference's ZeroPad2d copy, spatial.py:1020 / :1099, on every conv_spatial and
     every k>=3 Pool) + F.conv2d / F.*_pool2d (cuDNN / ATen) + autograd backward -- NCHW like the reference,
     cuDNN's default algorithm heuristics as the reference runs it (cudnn.benchmark's exhaustive search takes
     minutes at these sizes).  Two arms: bf16 storage, and fp32 storage with
@@ -236,87 +238,95 @@ def cudnn_baseline(torch, layers_unique, order, dev, steps, warmup, full_size_cu
     torch.backends.cuda.matmul.allow_tf32 = True
     try:
         for arm, dt in (("bf16", torch.bfloat16), ("fp32_tf32", torch.float32)):
-            _log("cudnn baseline arm %s" % arm)
-            max_in = max(u["in_shape"][1] * u["in_shape"][2] * u["in_shape"][3] for u in layers_unique.values())
-            max_out = max(u["out_shape"][1] * u["out_shape"][2] * u["out_shape"][3] for u in layers_unique.values())
-            sx = torch.randn(max_in, dtype=dt, device=dev)
-            sg = torch.randn(max_out, dtype=dt, device=dev) * 0.01
-            ws = {}
-            for key, u in layers_unique.items():
-                l = u["layer"]
-                if l["op"] == "conv":
-                    ws[key] = (torch.randn(l["K"], l["C"], l["R"], l["S"], dtype=dt, device=dev) * 0.05).requires_grad_(True)
+            try:   # one arm running out of memory keeps the other arm's numbers
+                _log("cudnn baseline arm %s" % arm)
+                max_in = max(u["in_shape"][1] * u["in_shape"][2] * u["in_shape"][3] for u in layers_unique.values())
+                max_out = max(u["out_shape"][1] * u["out_shape"][2] * u["out_shape"][3] for u in layers_unique.values())
+                sx = torch.randn(max_in, dtype=dt, device=dev)
+                sg = torch.randn(max_out, dtype=dt, device=dev) * 0.01
+                ws = {}
+                for key, u in layers_unique.items():
+                    l = u["layer"]
+                    if l["op"] == "conv":
+                        ws[key] = (torch.randn(l["K"], l["C"], l["R"], l["S"], dtype=dt, device=dev) * 0.05).requires_grad_(True)
 
-            def run_layer(key, split=1):
-                u = layers_unique[key]
-                l = u["layer"]
-                ish = list(u["in_shape"])
-                ish[2] //= split                      # `split` > 1: the top 1/split of the tile (see `splits` below)
-                n = ish[1] * ish[2] * ish[3]
-                x = sx[:n].view(ish).detach()
-                if not u["first"]:
-                    x.requires_grad_(True)
-                if l["op"] == "conv":
-                    xp = F.pad(x, (l["pad_w"], l["pad_w"], l["pad_h"], l["pad_h"])) if l.get("kind") == "conv_spatial" else x
-                    y = F.conv2d(xp, ws[key], None, (l["stride_h"], l["stride_w"]), 0)
-                else:
-                    xp = F.pad(x, (l["pad"],) * 4) if l["k"] >= 3 else x
-                    y = (F.max_pool2d if l["mode"] == "max" else F.avg_pool2d)(xp, l["k"], l["stride"], 0)
-                gy = sg[:y.numel()].view(y.shape)
-                if y.requires_grad:
-                    y.backward(gy)
-                x.grad = None
-                if l["op"] == "conv":
-                    ws[key].grad = None
+                def run_layer(key, split=1):
+                    u = layers_unique[key]
+                    l = u["layer"]
+                    ish = list(u["in_shape"])
+                    ish[2] //= split                      # `split` > 1: the top 1/split of the tile (see `splits` below)
+                    n = ish[1] * ish[2] * ish[3]
+                    x = sx[:n].view(ish).detach()
+                    if not u["first"]:
+                        x.requires_grad_(True)
+                    if l["op"] == "conv":
+                        xp = F.pad(x, (l["pad_w"], l["pad_w"], l["pad_h"], l["pad_h"])) if l.get("kind") == "conv_spatial" else x
+                        y = F.conv2d(xp, ws[key], None, (l["stride_h"], l["stride_w"]), 0)
+                    else:
+                        xp = F.pad(x, (l["pad"],) * 4) if l["k"] >= 3 else x
+                        y = (F.max_pool2d if l["mode"] == "max" else F.avg_pool2d)(xp, l["k"], l["stride"], 0)
+                    gy = sg[:y.numel()].view(y.shape)
+                    if y.requires_grad:
+                        y.backward(gy)
+                    x.grad = None
+                    if l["op"] == "conv":
+                        ws[key].grad = None
 
-            def ev(fn, reps):
-                torch.cuda.synchronize()
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record()
-                for _ in range(reps):
-                    fn()
-                e1.record()
-                torch.cuda.synchronize()
-                return e0.elapsed_time(e1) / reps
+                def ev(fn, reps):
+                    torch.cuda.synchronize()
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    for _ in range(reps):
+                        fn()
+                    e1.record()
+                    torch.cuda.synchronize()
+                    return e0.elapsed_time(e1) / reps
 
-            # per layer: one warm-up call, then 3 timed calls.  A convolution with a tensor of more than 2^31-1
-            # elements makes cuDNN's default heuristics fall back to kernels that take SECONDS per call (measured
-            # full-size on this B200: 3.9 s, 2.1 s, 11.3 s, 3.7 s for the four such layers, profiles/
-            # r2a_bench_n1_with_cudnn.json -- a 29.4 s step, and minutes of bench time).  Those layers are timed
-            # here on 1/split of the tile's rows and multiplied by split: cuDNN at its best, the comparison that
-            # is hardest on libspconv.
-            per, step_ms = [], 0.0
-            for key, u in layers_unique.items():
-                l = u["layer"]
-                if l["op"] == "conv":
-                    shape = "%d->%d %dx%d s%d @%dx%d" % (l["C"], l["K"], l["R"], l["S"], l["stride_h"], u["th"], u["tw"])
-                else:
-                    shape = "%s%d s%d C=%d @%dx%d" % (l["mode"], l["k"], l["stride"], l["C"], u["th"], u["tw"])
-                big = max(u["in_shape"][1] * u["in_shape"][2] * u["in_shape"][3],
-                          u["out_shape"][1] * u["out_shape"][2] * u["out_shape"][3])
-                split = 1
-                if l["op"] == "conv" and not full_size_cudnn:
-                    while big // split > 2**31 - 1:
-                        split *= 2
-                run_layer(key, split)
-                t1 = ev(lambda k=key, s_=split: run_layer(k, s_), 1)
-                ms = (t1 if t1 > 50.0 else ev(lambda k=key, s_=split: run_layer(k, s_), 3)) * split
-                e = dict(shape=shape, count=u["count"], fwd_bwd_ms=round(ms, 4))
-                if split > 1:
-                    e["timed_as"] = "%d x (1/%d of the rows)" % (split, split)
-                per.append(e)
-                step_ms += ms * u["count"]
-            out[arm] = dict(ms_per_step=step_ms, images_per_sec=1000.0 / step_ms, per_layer=per)
-            del sx, sg, ws
-            torch.cuda.empty_cache()
+                # per layer: one warm-up call, then 3 timed calls.  A convolution with a tensor of more than 2^31-1
+                # elements makes cuDNN's default heuristics fall back to kernels that take SECONDS per call (a step of
+                # tens of seconds, and minutes of bench time), and the largest fp32 layers do not fit in an 80 GB GPU
+                # next to the scratch tensors.  Those layers are timed here on 1/split of the tile's rows and multiplied
+                # by split: cuDNN at its best, the comparison that is hardest on libspconv.
+                per, step_ms = [], 0.0
+                for key, u in layers_unique.items():
+                    l = u["layer"]
+                    if l["op"] == "conv":
+                        shape = "%d->%d %dx%d s%d @%dx%d" % (l["C"], l["K"], l["R"], l["S"], l["stride_h"], u["th"], u["tw"])
+                    else:
+                        shape = "%s%d s%d C=%d @%dx%d" % (l["mode"], l["k"], l["stride"], l["C"], u["th"], u["tw"])
+                    big = max(u["in_shape"][1] * u["in_shape"][2] * u["in_shape"][3],
+                              u["out_shape"][1] * u["out_shape"][2] * u["out_shape"][3])
+                    split = 1
+                    if not full_size_cudnn:
+                        # input, padded input, their gradients, the output and its gradient, in this arm's dtype
+                        need = (4 * u["in_shape"][1] * u["in_shape"][2] * u["in_shape"][3] +
+                                2 * u["out_shape"][1] * u["out_shape"][2] * u["out_shape"][3]) * sx.element_size()
+                        free = torch.cuda.mem_get_info(dev)[0] + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+                        while (l["op"] == "conv" and big // split > 2**31 - 1) or need // split > free // 2:
+                            split *= 2
+                    run_layer(key, split)
+                    t1 = ev(lambda k=key, s_=split: run_layer(k, s_), 1)
+                    ms = (t1 if t1 > 50.0 else ev(lambda k=key, s_=split: run_layer(k, s_), 3)) * split
+                    e = dict(shape=shape, count=u["count"], fwd_bwd_ms=round(ms, 4))
+                    if split > 1:
+                        e["timed_as"] = "%d x (1/%d of the rows)" % (split, split)
+                    per.append(e)
+                    step_ms += ms * u["count"]
+                out[arm] = dict(ms_per_step=step_ms, images_per_sec=1000.0 / step_ms, per_layer=per)
+                del sx, sg, ws
+                torch.cuda.empty_cache()
+            except torch.cuda.OutOfMemoryError as e:
+                out[arm] = {"error": repr(e)[:300]}
+                sx = sg = ws = None
+                torch.cuda.empty_cache()
     finally:
         torch.backends.cudnn.benchmark, torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = old
     out["what"] = ("stock F.pad + F.conv2d / F.*_pool2d + autograd (cuDNN/ATen, NCHW, default heuristics) over the same "
                    "layer list and tile, CUDA events; fwd_bwd_ms = pad + fprop + dgrad + wgrad of one layer; "
                    "ms_per_step = sum over the layer list of count * fwd_bwd_ms; convolutions holding a tensor of more than 2^31-1 "
-                   "elements are timed on 1/split of the rows x split (entries with `timed_as`) because cuDNN takes "
-                   "seconds per call on them at full size (29.4 s/step, profiles/r2a_bench_n1_with_cudnn.json; "
-                   "--cudnn-full-size re-measures that)")
+                   "elements, and layers whose tensors would not fit in the free device memory, are timed on 1/split of "
+                   "the rows x split (entries with `timed_as`); cuDNN takes seconds per call on the former at full size "
+                   "(--cudnn-full-size measures that)")
     return out
 
 
@@ -397,6 +407,9 @@ def main():
     ap.add_argument("--cudnn-full-size", action="store_true",
                     help="time cuDNN on the whole tile even where a tensor exceeds 2^31-1 elements (adds minutes)")
     ap.add_argument("--no-model-stage", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (float32): the weight gradients "
+                         "of every conv in layer order, and a fixed sample of every layer's output and input gradient")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -437,6 +450,7 @@ def main():
     algo = _lib.SPC_ALGO_DIRECT if args.algo == "direct" else _lib.SPC_ALGO_AUTO
 
     # ---- build one module per distinct layer shape (weights shared by repeats) ------------------
+    torch.manual_seed(0)     # same weights (and host image) in every run: outputs comparable across builds
     uniq = {}
     order = []
     for l in d["layers"]:
@@ -490,6 +504,26 @@ def main():
             n *= s
         return buf[:n].view(shape)
 
+    # --dump-outputs: a fixed, seeded sample of every layer's output and input gradient, gathered in one extra, untimed
+    # step after the timed ones (no step changes weights or inputs, so it computes what every timed step computed);
+    # the weight gradients are kept whole in flat_grads
+    dump, dump_on = None, [False]
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        dump = []
+        for i, key in enumerate(order):
+            u = uniq[key]
+            ent = {}
+            for name, shape in (("y", u["out_shape"]), ("dx", u["in_shape"] if not u["first"] else None)):
+                if shape is None:
+                    continue
+                n = 1
+                for s_ in shape:
+                    n *= s_
+                idx = np.random.default_rng(1000 + i).choice(n, size=min(n, 8192), replace=False)
+                ent[name] = (torch.tensor(np.sort(idx), device=dev), torch.zeros(min(n, 8192), dtype=torch.float32, device=dev))
+            dump.append(ent)
+
     def step_body(from_host_image):
         """One pass of the hot path: every layer fwd + bwd, gradient flatten, allreduce / P."""
         off = 0
@@ -502,6 +536,11 @@ def main():
                 x.requires_grad_(True)
             y = u["mod"](x)
             y.backward(view(scratch_gy, u["out_shape"]))
+            if dump is not None and dump_on[0] and not from_host_image:
+                for name, t in (("y", y), ("dx", x.grad)):
+                    if name in dump[i]:
+                        idx, buf = dump[i][name]
+                        buf.copy_(t.detach().reshape(-1).index_select(0, idx))
             x.grad = None
             if u["layer"]["op"] == "conv":
                 w = u["mod"].weight
@@ -603,6 +642,22 @@ def main():
     clocks = sampler.stop(t_wall0, t_wall1) if sampler else None
     ms_e2e = timed(args.steps, True)
     _log("timed: %.2f ms/step, e2e %.2f ms/step" % (ms_total / args.steps, ms_e2e / args.steps))
+    if args.dump_outputs:
+        # every rank takes part in the step (halo exchange, allreduce); eager, with the graphs' memory released
+        graphs.clear()
+        g_dev = g_e2e = r_dev = r_e2e = None  # noqa: F841
+        torch.cuda.empty_cache()
+        dump_on[0] = True
+        step_body(False)
+        dump_on[0] = False
+        torch.cuda.synchronize()
+        if dump is not None:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "weight_grads.npy"), flat_grads.float().cpu().numpy())
+            for i, ent in enumerate(dump):
+                for name, (_, buf) in ent.items():
+                    np.save(os.path.join(args.dump_outputs, "layer%02d_%s.npy" % (i, name)), buf.cpu().numpy())
+            _log("outputs of the timed step written to %s" % args.dump_outputs)
 
     # ---- per-kernel timing pass: every distinct layer-op through the C ABI, CUDA events ----------
     def ev_time(fn, reps=3):
@@ -652,7 +707,7 @@ def main():
                     elif (l["K"] if nm == "fprop" else l["C"]) <= 128:
                         return "conv_tap_kernel"
                 if nm == "wgrad":
-                    return "pw_wgrad_pair_kernel" if (not taps and l["C"] >= 400 and l["K"] > 128) else "pw_wgrad_kernel"
+                    return "pw_wgrad_kernel"
                 return "pw_gemm_kernel"
 
             for nm, fn, (by, fl), is_tc in fns:
@@ -691,28 +746,6 @@ def main():
     roof["launches_per_step"] = dk["launches"]
     roof["peak_source"] = peak_src
     roof["share_of_step"] = dk["ms"] / sum(k["ms"] for k in kinds.values())
-    # DRAM traffic of that kernel from the committed ncu --set full capture (profiles/), for the
-    # heaviest single launch shape of the kernel, next to the same launch's algorithmic bytes
-    roof["traffic"] = None
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        cand = sorted((o for o in ops if o["kernel"] == dom_name), key=lambda o: -o["ms"] * o["count"])
-        for o in cand:
-            kk = o["shape"] + " " + o["op"]
-            if kk in tr:
-                roof["traffic"] = tr[kk]["dram_bytes"]
-                roof["traffic_launch"] = {"launch": kk, "algorithmic_bytes": o["bytes"], "event_ms": round(o["ms"], 4),
-                                          "achieved_GBps": round(o["bytes"] / o["ms"] / 1e6, 1), "ncu": tr[kk].get("source")}
-                break
-        # every launch shape an ncu --set full capture exists for, good and bad alike (VERDICT r1 #11)
-        roof["traffic_table"] = [
-            {"launch": o["shape"] + " " + o["op"], "kernel": o["kernel"], "algorithmic_bytes": o["bytes"],
-             "dram_bytes": tr[o["shape"] + " " + o["op"]]["dram_bytes"],
-             "ratio": round(tr[o["shape"] + " " + o["op"]]["dram_bytes"] / o["bytes"], 2),
-             "ncu": tr[o["shape"] + " " + o["op"]].get("source")}
-            for o in ops if (o["shape"] + " " + o["op"]) in tr]
-    except Exception:
-        pass
     # whole-step roofline (BASELINE.md: sum over layer-ops of max(F/P, B/BW))
     t_roof = sum(o["count"] * max(o["bytes"] / (hbm * 1e9), o["flops"] / (tfs * 1e12)) for o in ops)
     roof["step_roofline_ms"] = t_roof * 1e3
@@ -722,6 +755,12 @@ def main():
     per_layer = [dict(shape=o["shape"], op=o["op"], kernel=o["kernel"], count=o["count"], ms=round(o["ms"], 4),
                       GBps=round(o["bytes"] / o["ms"] / 1e6, 1), TFLOPs=round(o["flops"] / o["ms"] / 1e9, 1)) for o in ops]
 
+    if world == 1:
+        # the comparison arms below allocate tensors of their own: release the captured graphs (their private memory
+        # pool) and the timed path's scratch first, so that they fit next to it on an 80 GB GPU
+        graphs.clear()
+        g_dev = g_e2e = r_dev = r_e2e = scratch_x = scratch_gy = x = gy = w = ws = dw = None  # noqa: F841
+        torch.cuda.empty_cache()
     if rank == 0:
         cpu = None
         if not args.no_cpu_baseline and world == 1:
@@ -746,11 +785,12 @@ def main():
                 for o in ops:
                     ours[o["shape"]] = ours.get(o["shape"], 0.0) + o["ms"]
                 for arm in ("bf16", "fp32_tf32"):
-                    for r in cudnn[arm]["per_layer"]:
+                    for r in cudnn[arm].get("per_layer", []):
                         r["libspconv_ms"] = round(ours.get(r["shape"], float("nan")), 4)
-                cudnn["loses_to_cudnn_bf16"] = [r["shape"] for r in cudnn["bf16"]["per_layer"]
-                                                if r["libspconv_ms"] > r["fwd_bwd_ms"]]
-                cudnn["speedup_vs_cudnn_bf16_step"] = round(cudnn["bf16"]["ms_per_step"] / ms_step, 3)
+                if "per_layer" in cudnn["bf16"]:
+                    cudnn["loses_to_cudnn_bf16"] = [r["shape"] for r in cudnn["bf16"]["per_layer"]
+                                                    if r["libspconv_ms"] > r["fwd_bwd_ms"]]
+                    cudnn["speedup_vs_cudnn_bf16_step"] = round(cudnn["bf16"]["ms_per_step"] / ms_step, 3)
             except Exception as e:  # noqa: BLE001
                 cudnn = {"error": repr(e)[:300]}
         stage = None
@@ -763,7 +803,7 @@ def main():
             "vs_baseline": None, "dtype": args.dtype if args.dtype != "fp32" else "f32", "data": "synthetic",
             "config": {"workload": desc if not args.image else desc + " [debug image %d]" % image,
                        "global_batch": 1, "parallelism": "sp%d-%s" % (world, method), "tile": [image // gr, image // gc],
-                       "layers": len(order), "l2_policy": "inputs larger than L2 (every layer tensor >> 126 MB)",
+                       "layers": len(order), "l2_policy": "inputs larger than L2 (every layer tensor >> 50 MB)",
                        "note": "conv_spatial + Pool layers AND the 1x1 nn.Conv2d layers inside the spatial cells, "
                                "all through torchgems.spatial modules -> libspconv C ABI; BN/ReLU/concat excluded "
                                "(model_stage times the real cells with them)",

@@ -9,7 +9,7 @@ Per configuration it reports, as one JSON line on rank 0 (and appended to --out)
   us_exchange      device time of ONE exchange (post + collect kernels, no pad), CUDA events, max over ranks
   us_layer         halo_exchange_layer.forward (exchange + materialised padded tile, what the reference times)
   recv_bytes       bytes this rank receives per exchange (max over ranks)
-  GBps             recv_bytes / us_exchange   -- against 900 GB/s per direction (NVLink 5) / 770 measured peer copy
+  GBps             recv_bytes / us_exchange   -- against 900 GB/s (the frac_of_900GBps field; H100 NVLink 4 is 450 GB/s per direction)
 The reference's number for this path (benchmarks/communication/halo/README.md:24-43): 0.334 ms per exchange of
 a 1024^2 image in 4 vertical parts, halo_len 3, C = 1 -- `--reference-point` runs exactly that shape.
 Messages are small (a 2048-px edge of 64 bf16 channels is 256 KB), so the exchange is LATENCY-bound: us_exchange

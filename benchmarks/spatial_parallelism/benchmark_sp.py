@@ -9,7 +9,7 @@ Same command line as the reference's benchmarks/spatial_parallelism/benchmark_{r
         --slice-method square --split-size 2 --batch-size 1 --num-layers 18 --num-filters 416 --dtype bf16
 
 world size = spatial_size * P + split_size - spatial_size.  Extra flags of this script: --dtype
-{fp32,bf16} (bf16 puts the spatial convs on the tcgen05 kernels), --steps N (synthetic batches per
+{fp32,bf16} (bf16 puts the spatial convs on the wgmma kernels), --steps N (synthetic batches per
 epoch, default 10).  APP 3 (synthetic) needs no dataset; APP 1/2 use torchvision like the reference.
 """
 import math

@@ -1,5 +1,5 @@
 /*
- * spconv.h -- C ABI of libspconv.so: the B200 (sm_100a) spatial-parallel convolution engine
+ * spconv.h -- C ABI of libspconv.so: the H100 (sm_90a) spatial-parallel convolution engine
  * that sits under the torchgems Python API (mpi4dl_b200/torchgems/spatial.py).
  *
  * The reference (OSU-Nowlab/MPI4DL) has NO FFI: its hot path is Python calling
@@ -46,7 +46,7 @@ typedef struct {
   int32_t stride_h, stride_w;
   int32_t pad_h, pad_w;        /* == halo_len_height / halo_len_width */
   int32_t dtype;               /* SPC_F32 | SPC_BF16 */
-  int32_t algo;                /* SPC_ALGO_*; AUTO picks tcgen05 when the shape qualifies */
+  int32_t algo;                /* SPC_ALGO_*; AUTO picks the tensor-core (wgmma) path when the shape qualifies */
 } spc_conv_desc;
 
 typedef struct {
@@ -64,7 +64,7 @@ typedef struct {
 /* ---- library / device ------------------------------------------------------------------- */
 int         spc_version(void);
 const char* spc_last_error(void);
-/* sm count, compute capability major*10+minor; fails loudly when no sm_100 device is present */
+/* sm count, compute capability major*10+minor; fails loudly when the device is not sm_90 */
 int         spc_device_info(int device, int* sm_count, int* cc);
 /* number of kernels this library has launched since the last reset (bench.py's gpu_launches) */
 long long   spc_launch_count(int reset);
@@ -82,7 +82,7 @@ int spc_conv2d_fwd(const spc_conv_desc* d, const void* x, const spc_halo* halo, 
 /* The same convolution in two stream-ordered halves, so that the halo exchange (on a second
  * stream) overlaps the bulk of the compute -- the design the reference left as dead code
  * (spatial.py:415-866 make_tensor_halo_compute / compute_halo_exchange / merge_final_image):
- *   interior: the whole tile with ZERO padding (no halo needed; tcgen05 where the shape qualifies);
+ *   interior: the whole tile with ZERO padding (no halo needed; tensor cores where the shape qualifies);
  *   boundary: recompute the output rows/cols whose window reaches a received strip. */
 int spc_conv2d_fwd_interior(const spc_conv_desc* d, const void* x, const void* w, const void* bias,
                             void* y, void* workspace, size_t workspace_bytes, void* stream);
@@ -103,7 +103,7 @@ int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo
                      size_t workspace_bytes, void* stream);
 
 size_t spc_conv_workspace_bytes(const spc_conv_desc* d, int op /*0 fwd, 1 dgrad, 2 wgrad*/);
-/* 1 if the tcgen05 (tensor-core) kernel will be used for this op, else 0 (direct kernel) */
+/* 1 if the tensor-core (wgmma) kernel will be used for this op, else 0 (direct kernel); the name is historical */
 int    spc_conv_uses_tcgen05(const spc_conv_desc* d, int op);
 /* output extent of a tile: Ho = (H + 2*pad_h - R)/stride_h + 1 */
 void   spc_conv_out_shape(const spc_conv_desc* d, int* Ho, int* Wo);

@@ -1,8 +1,8 @@
-"""mpi4dl_b200 -- B200-native spatial-parallel convolution engine behind the torchgems API.
+"""mpi4dl_b200 -- H100-native (sm_90a) spatial-parallel convolution engine behind the torchgems API.
 
 Layout (only what the hot path needs):
-    csrc/            hand-written sm_100a CUDA kernels + the C ABI (include/spconv.h)
-    libspconv.so     built in-tree by build.py (nvcc -gencode arch=compute_100a,code=sm_100a)
+    csrc/            hand-written sm_90a CUDA kernels + the C ABI (include/spconv.h)
+    libspconv.so     built in-tree by build.py (nvcc -gencode arch=compute_90a,code=sm_90a)
     _lib.py          ctypes binding (no fallback: raises when the library is missing)
     torchgems/       host-side mirror of the reference's torchgems package for this path
 """

@@ -1,4 +1,4 @@
-"""Build libspconv.so (sm_100a) in-tree with nvcc.  Called by __graft_entry__.build()."""
+"""Build libspconv.so (sm_90a) in-tree with nvcc.  Called by __graft_entry__.build()."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libspconv.so")
 SOURCES = ["api.cu", "conv_direct.cu", "pool.cu", "halo.cu", "gemm_tc.cu", "conv_tap.cu", "wgrad_tap.cu", "bnrelu.cu"]
 NVCC_FLAGS = [
-    "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -41,7 +41,7 @@ def build_lib(force=False, verbose=False):
         if verbose:
             sys.stderr.write(out)
     if force or procs or _stale(LIB, objs):
-        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         subprocess.check_call(cmd)
     return LIB
 

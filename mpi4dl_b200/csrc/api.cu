@@ -1,6 +1,6 @@
 // api.cu -- C-ABI entry points for convolution (include/spconv.h) and algorithm dispatch.
 //
-// Dispatch: shapes the tcgen05 implicit-GEMM path supports (gemm_tc.cu) run there over the
+// Dispatch: shapes the wgmma implicit-GEMM path supports (gemm_tc.cu) run there over the
 // whole tile with zero padding; if the tile has neighbours, the thin output strips whose
 // receptive field reaches into a halo are then recomputed by the direct kernel, which reads the
 // received strips in place.  Interior compute therefore never waits on the halo exchange --
@@ -49,7 +49,7 @@ DirectConvParams fwd_params(const spc_conv_desc* d, const void* x, const spc_hal
 
 inline size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-// Boundary rect through the tcgen05 path: gather a 64-column-aligned patch of tile+halo around the
+// Boundary rect through the tensor-core path: gather a 64-column-aligned patch of tile+halo around the
 // rect, run the SAME fast convolution on that small image, scatter the rect back.  Stride 1 only.
 static bool patch_ok(const spc_conv_desc* d, int op) {
   if (d->dtype != SPC_BF16 || d->stride_h != 1 || d->stride_w != 1 || d->algo == SPC_ALGO_DIRECT) return false;
@@ -82,7 +82,7 @@ static int patch_fwd_rect(const spc_conv_desc* d, const void* x, const spc_halo*
   return launch_patch_scatter(O, y, d->N * d->K, Ho, Wo, q.H, q.W, y0, x0, rh, rw, ph, pw, d->dtype, st);
 }
 
-// dw += (halo pixels only) x (dy restricted to the rect), through the tcgen05 wgrad on a patch
+// dw += (halo pixels only) x (dy restricted to the rect), through the wgmma wgrad on a patch
 static int patch_wgrad_rect(const spc_conv_desc* d, const spc_halo* halo, const void* dy, float* dw, int y0, int y1,
                             int x0, int x1, cudaStream_t st) {
   if (y1 <= y0 || x1 <= x0) return SPC_OK;
@@ -107,16 +107,15 @@ static int patch_wgrad_rect(const spc_conv_desc* d, const spc_halo* halo, const 
   return tc_conv_wgrad(&q, P, G, dw, 1, ws, wsb, st);
 }
 
-// ---- halo fix-up of the tcgen05 paths: a small GEMM over the boundary outputs only ------------------------------
+// ---- halo fix-up of the tensor-core paths: a small GEMM over the boundary outputs only ------------------------------
 // After the interior pass ran the whole tile with zero padding, only the outputs whose window reaches a received
 // strip are wrong (P_b of them: a few rows / columns).  fprop: V[(c,r,s)][p] = im2col of tile + strips over those
-// P_b outputs, then ONE pointwise GEMM  O[K][P_b] = w[K][C*R*S] * V (+bias)  on the tcgen05 kernel -- the filter tensor
+// P_b outputs, then ONE pointwise GEMM  O[K][P_b] = w[K][C*R*S] * V (+bias)  on the wgmma kernel -- the filter tensor
 // IS that matrix -- and a scatter that overwrites them.  wgrad: the halo pixels' share is linear, so with V taken
 // from the HALO-ONLY view  dW[K][C*R*S] += dY_b[K][P_b] * V^T  (pw_wgrad_kernel accumulating straight into dw).
-// Round 1 gathered a 64-column-aligned patch around every boundary rectangle and re-ran the convolution on it
-// (3 launches per rectangle, up to 4 rectangles; strided layers fell to the direct kernel on thin strips): +0.18 ms
-// per 1x7 fprop and +0.59 ms per wgrad on the 1024x128 tiles of an 8-GPU run (profiles/r2_halo_cost_n8.txt) -- more
-// than the interior pass itself; now +0.07 / +0.08 ms (profiles/r2_halo_cost_n8_v2.txt).
+// The alternative (SPC_BOUNDARY_V1=1) gathers a 64-column-aligned patch around every boundary rectangle and re-runs the
+// convolution on it: 3 launches per rectangle, up to 4 rectangles, and strided layers fall to the direct kernel on thin
+// strips -- on small tiles that can cost more than the interior pass itself.
 static bool boundary_rects(const spc_conv_desc* d, const spc_halo* halo, int Ho, int Wo, BoundaryRects* b) {
   const int top = min(Ho, ceil_div(d->pad_h, d->stride_h));
   int bot0 = ceil_div(d->H + d->pad_h - d->R + 1, d->stride_h);      // first output row touching the bottom halo
@@ -259,7 +258,7 @@ static int fwd_interior(const spc_conv_desc* d, const void* x, const void* w, co
                         size_t workspace_bytes, cudaStream_t st) {
   const bool tc = spc_conv_uses_tcgen05(d, 0);
   if (d->algo == SPC_ALGO_TCGEN05 && !tc) {
-    set_error("conv_fwd: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tcgen05 path");
+    set_error("conv_fwd: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
     return SPC_EUNSUPPORTED;
   }
   if (tc) return tc_conv_fwd(d, x, w, bias, y, workspace, workspace_bytes, st);
@@ -307,7 +306,7 @@ int spc_conv2d_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void
   SPC_REQUIRE(dy && w && dx, "conv_dgrad: null tensor pointer");
   const bool tc = spc_conv_uses_tcgen05(d, 1);
   if (d->algo == SPC_ALGO_TCGEN05 && !tc) {
-    set_error("conv_dgrad: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tcgen05 path");
+    set_error("conv_dgrad: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
     return SPC_EUNSUPPORTED;
   }
   if (tc) return tc_conv_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
@@ -367,7 +366,7 @@ int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo
   }
   const bool tc = spc_conv_uses_tcgen05(d, 2);
   if (d->algo == SPC_ALGO_TCGEN05 && !tc) {
-    set_error("conv_wgrad: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tcgen05 path");
+    set_error("conv_wgrad: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
     return SPC_EUNSUPPORTED;
   }
   DirectWgradParams p{};

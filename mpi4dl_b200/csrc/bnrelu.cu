@@ -175,7 +175,7 @@ int bn_geom(int N, int C, long long HW, BnGeom* g, int* grid) {
   g->C = C; g->HW = HW; g->planes = (long long)N * C;
   g->chunks = (int)((HW + BN_CHUNK - 1) / BN_CHUNK);
   g->items = g->planes * g->chunks;
-  long long b = g->items < 148 * 8 ? g->items : 148 * 8;
+  long long b = g->items < 132 * 8 ? g->items : 132 * 8;
   *grid = (int)b;
   return SPC_OK;
 }

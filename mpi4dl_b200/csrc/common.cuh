@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for libspconv (sm_100a).
+// common.cuh -- shared device helpers for libspconv (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -162,7 +162,7 @@ int tc_pw_fwd(const void* w, int ld, int M, int Cin, const void* x, const void* 
               cudaStream_t st);
 int tc_pw_wgrad(const void* x, const void* dy, float* dw, int K, int C, int P, cudaStream_t st);
 
-// ---- tcgen05 pointwise GEMM path: gemm_tc.cu ---------------------------------------------
+// ---- wgmma pointwise GEMM path: gemm_tc.cu -----------------------------------------------
 bool tc_supported(const spc_conv_desc* d, int op);
 size_t tc_workspace_bytes(const spc_conv_desc* d, int op);
 int tc_conv_fwd(const spc_conv_desc* d, const void* x, const void* w, const void* bias, void* y,

@@ -1,7 +1,7 @@
-// conv_direct.cu -- CUDA-core (FFMA) direct convolution kernels for sm_100a.
+// conv_direct.cu -- CUDA-core (FFMA) direct convolution kernels for sm_90a.
 //
 // Role in the engine: the shape-complete path.  Every conv_spatial configuration the reference
-// accepts (spatial.py:25-155: any odd RxS, stride 1/2, "same" padding) runs here; the tcgen05
+// accepts (spatial.py:25-155: any odd RxS, stride 1/2, "same" padding) runs here; the wgmma
 // GEMM path (gemm_tc.cu) takes over for the shapes that dominate the AmoebaNet-D / ResNet
 // workloads.  It also computes the thin boundary strips whose receptive field touches
 // neighbour halos, reading halo strips in place (TileView) instead of materialising the padded
@@ -362,7 +362,7 @@ int launch_wgrad_halo(const DirectWgradParams& p, int dtype, cudaStream_t st) {
   if (npix <= 0) return SPC_OK;
   const int kblocks = ceil_div(p.K, 16), cblocks = ceil_div(p.in.C, 16);
   int chunks = (int)((npix + 255) / 256);
-  const int max_chunks = (148 * 8 + kblocks * cblocks - 1) / (kblocks * cblocks);
+  const int max_chunks = (132 * 8 + kblocks * cblocks - 1) / (kblocks * cblocks);
   if (chunks > max_chunks) chunks = max_chunks;
   if (chunks < 1) chunks = 1;
   const int pix_per_cta = (int)((npix + chunks - 1) / chunks);
@@ -387,8 +387,8 @@ int launch_wgrad_direct(const DirectWgradParams& p_in, int dtype, cudaStream_t s
   const int tiles_x = ceil_div(p.rW, WG_TW), tiles_y = ceil_div(p.rH, WG_TH);
   const int kblocks = ceil_div(p.K, WG_KB), cblocks = ceil_div(p.in.C, WG_CB);
   const int total_tiles = p.in.N * tiles_x * tiles_y;
-  // enough CTAs for ~4 waves of 148 SMs x 2 resident CTAs, but at least 8 tiles each
-  int want = (148 * 8) / (kblocks * cblocks);
+  // enough CTAs for ~4 waves of 132 SMs x 2 resident CTAs, but at least 8 tiles each
+  int want = (132 * 8) / (kblocks * cblocks);
   if (want < 1) want = 1;
   int tiles_per_cta = ceil_div(total_tiles, want);
   if (tiles_per_cta < 8) tiles_per_cta = 8;

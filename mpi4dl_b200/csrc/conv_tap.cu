@@ -1,4 +1,4 @@
-// conv_tap.cu -- tcgen05 implicit-GEMM kernel for the multi-tap ("same", stride 1) convolutions of the
+// conv_tap.cu -- wgmma implicit-GEMM kernel for the multi-tap ("same", stride 1) convolutions of the
 // spatial stages: 1x7 / 7x1 (AmoebaNet-D cells), 3x3 (ResNet), fprop and -- with the rotated,
 // transposed filter -- dgrad.  Replaces round 1's approach (S column-shifted COPIES of the input in HBM
 // because TMA tile loads need 16-byte aligned inner coordinates, then one TMA load per tap: 8x the
@@ -10,13 +10,13 @@
 //   * vertical taps (r) are just different row blocks of that buffer (UMMA descriptor start address);
 //   * horizontal taps (s) are formed IN SHARED MEMORY by four "shifter" warps: each 16-byte chunk of the
 //     operand tile of tap (r, s) is a funnel shift of the aligned 24-pixel window around it, written in
-//     the swizzled MN-major layout tcgen05.mma reads.  Nothing shifted ever exists in HBM or L2;
+//     the swizzled MN-major layout wgmma reads.  Nothing shifted ever exists in HBM or L2;
 //   * weights stay resident in shared memory when they fit, else stream through a small ring;
-//   * accumulators (NB*64 pixels x 128 channels, double buffered) live in TMEM; epilogue threads own one
-//     output channel each and store contiguous NCHW runs straight from registers.
+//   * accumulators (128 pixels x 128 channels) live in the registers of two consumer warpgroups, which issue the
+//     wgmma and write each tile row through a swizzled staging block and a TMA store.
 //
-// Warp roles (448 threads): 0 = TMA producer (activation row blocks and weight blocks, interleaved), 1 = MMA issuer
-// (+TMEM alloc), 2..5 = epilogue, 6..13 = shifter.  All hand-offs are mbarriers; persistent CTAs, one per SM.
+// Warp roles (640 threads): 0 = TMA producer (activation row blocks and weight blocks, interleaved), 4..11 = two
+// consumer warpgroups, 12..19 = shifter.  All hand-offs are mbarriers; persistent CTAs, one per SM.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -32,7 +32,7 @@ int tc_sm_count();
 
 namespace {
 
-constexpr int TAP_THREADS = 448;
+constexpr int TAP_THREADS = 640;
 constexpr int BLK = 8192;          // one operand block: [64 ch][64 px] bf16, 128-byte rows, SWIZZLE_128B
 constexpr int RAW_SHIFT_ROW = 160;  // raw row block of the shift path: [cbox ch][80 px], dense rows of 160 B
 constexpr int MAXRING = 8;
@@ -136,7 +136,10 @@ struct ShiftRow {
   }
 };
 
-template <int NB, int S>
+// Warp roles (640 threads): warp 0 = TMA producer (warps 1-3 idle), warpgroups 1-2 = wgmma consumers + epilogue (rows
+// [64 g, 64 g + 64) of the output channels each), warps 12-19 = shifter.  KS = 16-channel k-steps per chunk (cbox / 16):
+// a compile-time count, so that no wgmma sits under a data-dependent branch (ptxas would serialise all of them).
+template <int NB, int S, int KS>
 __global__ void __launch_bounds__(TAP_THREADS, 1)
 conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
                 const __grid_constant__ CUtensorMap tmap_y, const TapParams p) {
@@ -159,32 +162,21 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
   uint64_t* a_empty = a_full + MAXRING;
   uint64_t* op_full = a_empty + MAXRING;
   uint64_t* op_empty = op_full + MAXRING;
-  uint64_t* tfull = op_empty + MAXRING;
-  uint64_t* tempty = tfull + 2;
-  uint64_t* a_res_full = tempty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(a_res_full + 1);
+  uint64_t* a_res_full = op_empty + MAXRING;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull[i], 1);
-      mbar_init(&tempty[i], 128);
-    }
     for (int i = 0; i < MAXRING; ++i) {
       mbar_init(&raw_full[i], 1);
-      mbar_init(&raw_empty[i], SHIFT ? SHIFT_THREADS : 1);   // shift path: released by the shifter threads
-      mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1);
-      mbar_init(&op_full[i], SHIFT_THREADS); mbar_init(&op_empty[i], 1);
+      mbar_init(&raw_empty[i], SHIFT ? SHIFT_THREADS : 2);   // shift path: the shifter threads, else the two consumers
+      mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 2);
+      mbar_init(&op_full[i], SHIFT_THREADS); mbar_init(&op_empty[i], 2);
     }
     mbar_init(a_res_full, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
 #define TAP_TILE_DECODE(t)                                        \
   const int tw_ = (t) % p.tiles_w;                                \
@@ -258,61 +250,16 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
         ct = nt; ckc = nkc;
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      constexpr uint32_t IDESC = umma_idesc_bf16(128, NPIX, /*a_mn=*/0, /*b_mn=*/1);
-      if (p.a_resident) { mbar_wait(a_res_full, 0); tc_fence_after(); }
-      RingState rb, ra, ro;
-      int acc = 0, aph = 0;
-      for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
-        mbar_wait(&tempty[acc], aph ^ 1);
-        tc_fence_after();
-        for (int kc = 0; kc < p.kchunks; ++kc) {
-          if (!SHIFT && !(p.dbg & 2)) { mbar_wait(&raw_full[rb.s], rb.ph); tc_fence_after(); }
-          const int nsteps = min(4, (p.Cin - kc * 64 + 15) / 16);
-          for (int tap = 0; tap < taps; ++tap) {
-            uint32_t sb;
-            const int si = tap % S;                                   // filter column (compile-time S)
-            if (SHIFT) {
-              if (!p.group || si == 0) mbar_wait(&op_full[ro.s], ro.ph);
-              sb = smem_u32(op_base + ro.s * slot_bytes + (p.group ? si * NB * p.opblk : 0));
-            } else {
-              sb = smem_u32(raw_base + (rb.s * p.rows_raw + tap) * RAW_BLK);   // S == 1: tap == filter row
-            }
-            uint32_t sa;
-            if (p.a_resident) {
-              sa = smem_u32(a_base + (tap * p.kchunks + kc) * p.a_blk);
-            } else {
-              if (!(p.dbg & 1)) mbar_wait(&a_full[ra.s], ra.ph);
-              sa = smem_u32(a_base + ra.s * p.a_blk);
-            }
-            tc_fence_after();
-            for (int ks = 0; ks < nsteps; ++ks) {
-              // B: MN-major SW128, 16 channels = two 8-row groups (SBO 1024 B); 64-pixel blocks (= tile rows) at LBO
-              const uint64_t bdesc = umma_desc(sb + ks * 2048, SHIFT ? p.opblk : RAW_BLK, 1024);
-              // A: K-major SW128, 8-row groups at SBO 1024 B; +32 B per 16-channel k-step
-              const uint64_t adesc = umma_desc(sa + ks * 32, 16, 1024);
-              umma_bf16(tmem_base + acc * NPIX, adesc, bdesc, IDESC, (kc | tap | ks) ? 1u : 0u);
-            }
-            if (SHIFT && (!p.group || si == S - 1)) { umma_commit(&op_empty[ro.s]); ro.next(p.ops); }
-            if (!p.a_resident) { if (!(p.dbg & 1)) umma_commit(&a_empty[ra.s]); ra.next(p.ast); }
-          }
-          if (!SHIFT) { if (!(p.dbg & 2)) umma_commit(&raw_empty[rb.s]); rb.next(p.rawb); }
-        }
-        umma_commit(&tfull[acc]);
-        if (++acc == 2) { acc = 0; aph ^= 1; }
-      }
-    }
-  } else if (warp >= 6) {
+  } else if (warp >= 12) {
     // ================= shifter: raw row blocks -> swizzled operand tile of tap (r, s) =================
     if (SHIFT) {
-      const int tid = threadIdx.x - 6 * 32;   // 0..255
+      const int tid = threadIdx.x - 12 * 32;   // 0..255
       RingState rb, ro;
       for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
         for (int kc = 0; kc < p.kchunks; ++kc) {
           if (!(p.dbg & 2)) mbar_wait(&raw_full[rb.s], rb.ph);
-          const int cv = (p.dbg & 8) ? 0 : min(64, (p.Cin - kc * 64 + 15) & ~15);      // channels the MMA reads of this chunk
+          // every channel row the MMA reads (KS * 16 = cbox): rows past Cin are zero, TMA zero-fills them in the raw box
+          const int cv = (p.dbg & 8) ? 0 : p.cbox;
           const uint8_t* rawb = raw_base + rb.s * p.rows_raw * RAW_BLK;
           for (int r = 0; r < p.R; ++r)
             ShiftRow<NB, S, 0>::run(rawb + r * RAW_BLK, RAW_BLK, cv, tid, op_base, p.opblk, p.group, op_full, op_empty, ro, p.ops);
@@ -321,62 +268,102 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
         }
       }
     }
-  } else if (warp >= 2 && warp <= 5) {
-    // ================= epilogue: TMEM -> registers -> NCHW runs =================
-    const int quarter = warp & 3;
-    const int k = quarter * 32 + lane;                 // output channel = TMEM lane
-    const float bias = (k < p.M && p.bias) ? __bfloat162float(p.bias[k]) : 0.f;
-    const bool leader = threadIdx.x == 64;
-    int acc = 0, aph = 0;
+  } else if (threadIdx.x >= 128) {
+    // ================= consumers: wgmma over (chunk, tap), then registers -> NCHW rows =================
+    const int wg = (threadIdx.x >> 7) - 1;
+    const int w4 = (threadIdx.x >> 5) & 3;
+    const bool wg_lead = (threadIdx.x & 127) == 0;
+    const bool leader = threadIdx.x == 128;    // issues the TMA stores
+    float acc[NPIX / 2];
+    if (p.a_resident) mbar_wait(a_res_full, 0);
+    RingState rb, ra, ro;
     for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
       TAP_TILE_DECODE(t)
-      mbar_wait(&tfull[acc], aph);
-      tc_fence_after();
-#pragma unroll 1
+      // ring slots read by the last committed wgmma group; released once the next group is committed and the
+      // previous one has completed (wgmma_wait<1>)
+      int rel_op = -1, rel_a = -1, rel_raw = -1;
+      for (int kc = 0; kc < p.kchunks; ++kc) {
+        if (!SHIFT && !(p.dbg & 2)) mbar_wait(&raw_full[rb.s], rb.ph);
+        for (int tap = 0; tap < taps; ++tap) {
+          uint32_t sb;
+          const int si = tap % S;                                   // filter column (compile-time S)
+          if (SHIFT) {
+            if (!p.group || si == 0) mbar_wait(&op_full[ro.s], ro.ph);
+            sb = smem_u32(op_base + ro.s * slot_bytes + (p.group ? si * NB * p.opblk : 0));
+          } else {
+            sb = smem_u32(raw_base + (rb.s * p.rows_raw + tap) * RAW_BLK);   // S == 1: tap == filter row
+          }
+          uint32_t sa;
+          if (p.a_resident) {
+            sa = smem_u32(a_base + (tap * p.kchunks + kc) * p.a_blk);
+          } else {
+            if (!(p.dbg & 1)) mbar_wait(&a_full[ra.s], ra.ph);
+            sa = smem_u32(a_base + ra.s * p.a_blk);
+          }
+          wgmma_fence();
+#pragma unroll
+          for (int ks = 0; ks < KS; ++ks) {
+            // B: MN-major SW128, 16 channels = two 8-row groups (SBO 1024 B); 64-pixel blocks (= tile rows) at LBO
+            const uint64_t bdesc = gmma_desc(sb + ks * 2048, SHIFT ? p.opblk : RAW_BLK, 1024);
+            // A: K-major SW128, 8-row groups at SBO 1024 B, this warpgroup's 64 rows 8 KB in; +32 B per k-step
+            const uint64_t adesc = gmma_desc(sa + wg * 8192 + ks * 32, 16, 1024);
+            Wgmma<NPIX, 1>::mma(acc, adesc, bdesc, (kc | tap | ks) ? 1u : 0u);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (wg_lead) {
+            if (rel_op >= 0) mbar_arrive(&op_empty[rel_op]);
+            if (rel_a >= 0 && !(p.dbg & 1)) mbar_arrive(&a_empty[rel_a]);
+            if (rel_raw >= 0 && !(p.dbg & 2)) mbar_arrive(&raw_empty[rel_raw]);
+          }
+          rel_op = rel_a = rel_raw = -1;
+          if (SHIFT && (!p.group || si == S - 1)) { rel_op = ro.s; ro.next(p.ops); }
+          if (!p.a_resident) { rel_a = ra.s; ra.next(p.ast); }
+          if (!SHIFT && tap == taps - 1) { rel_raw = rb.s; rb.next(p.rawb); }
+        }
+      }
+      wgmma_wait<0>();
+      reg_fence(acc);
+      if (wg_lead) {
+        if (rel_op >= 0) mbar_arrive(&op_empty[rel_op]);
+        if (rel_a >= 0 && !(p.dbg & 1)) mbar_arrive(&a_empty[rel_a]);
+        if (rel_raw >= 0 && !(p.dbg & 2)) mbar_arrive(&raw_empty[rel_raw]);
+      }
+      const int r0 = 64 * wg + 16 * w4 + (lane >> 2);   // fragment rows (output channels) r0 and r0 + 8
+      const float b0 = (r0 < p.M && p.bias) ? __bfloat162float(p.bias[r0]) : 0.f;
+      const float b1 = (r0 + 8 < p.M && p.bias) ? __bfloat162float(p.bias[r0 + 8]) : 0.f;
+#pragma unroll
       for (int j = 0; j < NB; ++j) {
         // the TMA store that last read the staging buffer must be done reading it
         if (leader) tma_store_wait_read<0>();
-        named_bar_sync(1, 128);
+        named_bar_sync(1, 256);
 #pragma unroll
-        for (int cc = 0; cc < 2; ++cc) {
-          uint32_t r[32];
-          tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + acc * NPIX + j * 64 + cc * 32, r);
-          tmem_ld_wait();
-          uint8_t* rowp = stage_base + k * 128;           // thread = output channel = one 128-byte row of the box
+        for (int q = 0; q < 8; ++q) {                   // 8-pixel column group of tile row j
 #pragma unroll
-          for (int v = 0; v < 4; ++v) {
-            uint4 o;
-            o.x = pack_bf16x2(__uint_as_float(r[8 * v + 0]) + bias, __uint_as_float(r[8 * v + 1]) + bias);
-            o.y = pack_bf16x2(__uint_as_float(r[8 * v + 2]) + bias, __uint_as_float(r[8 * v + 3]) + bias);
-            o.z = pack_bf16x2(__uint_as_float(r[8 * v + 4]) + bias, __uint_as_float(r[8 * v + 5]) + bias);
-            o.w = pack_bf16x2(__uint_as_float(r[8 * v + 6]) + bias, __uint_as_float(r[8 * v + 7]) + bias);
-            const int chunk = (cc * 4 + v) ^ (k & 7);     // SWIZZLE_128B: 16-byte chunk ^ (row % 8)
-            *reinterpret_cast<uint4*>(rowp + chunk * 16) = o;
+          for (int h = 0; h < 2; ++h) {
+            const int r = r0 + 8 * h;
+            const float bias = h ? b1 : b0;
+            const int i = 4 * (8 * j + q) + 2 * h;
+            const uint32_t v = pack_bf16x2(acc[i] + bias, acc[i + 1] + bias);
+            // SWIZZLE_128B: 16-byte chunk ^ (row % 8)
+            *reinterpret_cast<uint32_t*>(stage_base + r * 128 + ((q ^ (r & 7)) << 4) + (lane & 3) * 4) = v;
           }
         }
-        if (j == NB - 1) {                                // accumulator fully read: the MMA may reuse it
-          tc_fence_before();
-          mbar_arrive(&tempty[acc]);
-        }
         fence_proxy_async();                              // smem writes -> visible to the TMA (async proxy)
-        named_bar_sync(1, 128);
+        named_bar_sync(1, 256);
         // rows past the image and channels past M are clipped by the tensor map
         if (leader && !(p.dbg & 4) && h0 + j < p.H) {
           tma_store_4d(&tmap_y, stage_base, w0, h0 + j, 0, n_);
           tma_store_commit();
         }
       }
-      if (++acc == 2) { acc = 0; aph ^= 1; }
     }
     if (leader) tma_store_wait_read<0>();
   }
 #undef TAP_TILE_DECODE
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
-constexpr int TAP_SMEM_LIMIT = 222 * 1024;
+constexpr int TAP_SMEM_LIMIT = 222 * 1024;   // of H100's 227 KB per block
 constexpr int TAP_SMEM_AUX = 1024 /*align*/ + 1024 /*barriers*/;
 
 inline int round_up_i(int a, int b) { return (a + b - 1) / b * b; }
@@ -404,8 +391,8 @@ bool plan_tap(int M, int Cin, int R, int S, int H, int W, int N, TapPlan* out) {
   // buffers follow the A region (always >= 16 KB)
   p.opblk = p.cbox * 128;
   const int budget_ops = budget - STAGE_BYTES;
-  for (int NB = 4; NB >= 2; NB -= 2) {
-    if (NB == 4 && H < 4) continue;
+  // one tile = 2 rows of 64 pixels: 128 accumulator columns, 64 fp32 registers per consumer thread
+  for (int NB = 2; NB >= 2; NB -= 2) {
     p.rows_raw = NB + R - 1;
     const int raw_buf = p.rows_raw * raw_blk;                   // one raw buffer (all row blocks of a chunk)
     const int a_res = taps * p.kchunks * p.a_blk;
@@ -435,10 +422,10 @@ bool plan_tap(int M, int Cin, int R, int S, int H, int W, int N, TapPlan* out) {
   return false;
 }
 
-template <int NB, int S>
+template <int NB, int S, int KS>
 int launch_tap(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& ty, const TapParams& p, int smem,
                cudaStream_t st) {
-  auto kern = conv_tap_kernel<NB, S>;
+  auto kern = conv_tap_kernel<NB, S, KS>;
   static bool attr_set = false;
   if (!attr_set) {
     SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TAP_SMEM_LIMIT));
@@ -497,8 +484,10 @@ int run_conv_tap_v2(const __nv_bfloat16* wp, int Mpad, int Cpad, const __nv_bflo
     int rc = make_tmap_ex(&ty, y, 4, dims, strides, box, 1);
     if (rc) return rc;
   }
-#define TAP_CASE(nb, s) if (pl.NB == nb && S == s) return launch_tap<nb, s>(tw, tx, ty, p, pl.smem, st);
-  TAP_CASE(2, 1) TAP_CASE(4, 1) TAP_CASE(2, 3) TAP_CASE(4, 3) TAP_CASE(2, 5) TAP_CASE(4, 5) TAP_CASE(2, 7) TAP_CASE(4, 7)
+#define TAP_CASE(s, ks) if (S == s && p.cbox == 16 * ks) return launch_tap<2, s, ks>(tw, tx, ty, p, pl.smem, st);
+#define TAP_CASES(s) TAP_CASE(s, 1) TAP_CASE(s, 2) TAP_CASE(s, 3) TAP_CASE(s, 4)
+  TAP_CASES(1) TAP_CASES(3) TAP_CASES(5) TAP_CASES(7)
+#undef TAP_CASES
 #undef TAP_CASE
   set_error("tap conv: unsupported filter width %d", S);
   return SPC_EUNSUPPORTED;

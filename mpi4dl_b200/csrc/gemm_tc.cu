@@ -1,5 +1,6 @@
-// gemm_tc.cu -- tcgen05 (5th-gen tensor core) GEMM path for the 1x1 ("pointwise") convolutions
-// that carry ~90% of the HBM traffic of the AmoebaNet-D / ResNet spatial stages (SURVEY 8d).
+// gemm_tc.cu -- Hopper wgmma GEMM path for the 1x1 ("pointwise") convolutions that carry most of the HBM
+// traffic of the AmoebaNet-D / ResNet spatial stages (SURVEY 8d), and -- over column-shifted copies of the
+// input -- for the multi-tap ones.
 //
 // NCHW makes a 1x1 convolution a plain GEMM per image with NO layout change:
 //     fprop : Y[K x P] = W [K x C] * X [C x P]        P = H*W pixels, contiguous in memory
@@ -7,17 +8,16 @@
 //     wgrad : dW[K x C] = dY[K x P] * X[C x P]^T       (reduction over pixels)
 // fprop/dgrad: A = (padded) weights, K-major, TMA box {64 ch, 128 rows}, SWIZZLE_128B;
 //              B = activations read IN PLACE by TMA as an MN-major operand: [ch][64 px] rows of 128 B,
-//              SWIZZLE_128B; accumulator D[128 out-ch x BN px] lives in TMEM.  The epilogue goes
-//              TMEM -> registers -> swizzled staging block in smem -> TMA store.
+//              SWIZZLE_128B; accumulator D[128 out-ch x 128 px] in the registers of two consumer warpgroups.
+//              The epilogue goes registers -> swizzled staging block in smem -> TMA store.
 // wgrad:       both operands K-major straight from NCHW (pixels = reduction dim, contiguous).
 // Box shapes:  a [64 ch][64 px] box touches 64 channel planes = 64 different 2 MB pages, and with plane strides
-//              of 8..32 MB they alias in the translation cache: every 128 bytes cost a page walk (4.3 TB/s
-//              ceiling, DESIGN.md "Address translation").  Layers with multi-page planes therefore move ONE
+//              of 8..32 MB they alias in the translation cache.  Layers with multi-page planes therefore move ONE
 //              5-d box per stage, dims (64 px, 8 ch, P/64 px blocks, C/8 ch groups, image): the TMA unit walks
 //              8 planes at a time and visits all pixel blocks of each before moving on; smem layout
-//              [group][block][8 ch][128 B], which the UMMA descriptors express through LBO / SBO.
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM alloc),
-// warps 2..5 = epilogue.  Persistent CTAs, one per SM (wgrad for >= 400 input channels: CTA pairs, cta_group::2).
+//              [group][block][8 ch][128 B], which the GMMA descriptors express through LBO / SBO.
+// Warp roles (384 threads): warp 0 = TMA producer, warpgroups 1 and 2 = wgmma consumers + epilogue.
+// Persistent CTAs, one per SM.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -39,11 +39,10 @@ int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, in
 
 namespace {
 
-constexpr int TC_THREADS = 192;
+constexpr int TC_THREADS = 384;
 constexpr int BK = 64;                 // channels per pipeline stage (one 128-byte swizzle row of A)
 constexpr int A_BLK_BYTES = 128 * BK * 2;   // one 128-row M block of A per stage: 16 KB
 constexpr int B_BLK_BYTES = BK * 64 * 2;    // one 64-pixel block of B per stage: 8 KB
-constexpr int TMEM_COLS = 512;
 
 // ---- host: TMA descriptor encode (driver entry point fetched through the runtime) -------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -74,7 +73,7 @@ int make_tmap_sw(CUtensorMap* m, const void* base, int rank, const uint64_t* dim
   static thread_local bool ctx_bound = false;
   if (!ctx_bound) {
     if (cudaFree(nullptr) != cudaSuccess) {
-      set_error("tcgen05 conv: no CUDA context on this thread");
+      set_error("wgmma conv: no CUDA context on this thread");
       return SPC_ECUDA;
     }
     ctx_bound = true;
@@ -123,8 +122,8 @@ __global__ void repack_weights_kernel(const __nv_bfloat16* __restrict__ w, __nv_
 }
 
 // ---- fprop / dgrad kernel -----------------------------------------------------------------------
-constexpr int BN_DEFAULT = 128;               // pixels per tile (two 64-pixel swizzle blocks); 256 in the wide-N variant
-constexpr int OUT_BUF_BYTES = 128 * 128 * 2;  // epilogue staging: one 128-channel block of 128 pixels of a tile
+constexpr int BN = 128;                       // pixels per tile (two 64-pixel swizzle blocks)
+constexpr int OUT_BUF_BYTES = 128 * 128 * 2;  // epilogue staging: one 128-channel block of the tile's 128 pixels
 constexpr int MAX_STAGES = 8;
 
 struct PwParams {
@@ -144,32 +143,24 @@ struct PwParams {
   int rowmul;                  // input row = rowmul * output row + tap row offset (2 for stride-2 convs)
   int tgroup;                  // consecutive tiles handled back-to-back by one CTA (DRAM page locality)
   const __nv_bfloat16* bias;   // [M] or null
-  __nv_bfloat16* y;            // output base [N][M][P] (coalesced-store epilogue)
-  int epi_stg;                 // 1: staged tile leaves with per-thread 16-B stores (full 128-B lines), 0: TMA store
   int x5, y5;                  // 1: activations / outputs move as ONE 5-d box per tile whose traversal order is
                                // (8-channel group, 64-pixel block, channel, pixel): the TMA unit touches 8 channel
                                // planes (2 MB pages each) at a time and visits both pixel blocks of each before moving
                                // on, instead of walking 64 / 128 planes per pixel block (address-translation reach)
-  int stationary_ok;           // host: stationary weights allowed with several output-channel groups
-  int xbox, ybox;              // channel rows per TMA load / store box (64 / 128 = one box per 64-pixel block; smaller
-                               // boxes walk FEWER channel planes -- 2 MB pages -- between the two pixel blocks of a tile)
 };
 
-// EXT = false compiles the round-2 options (5-d boxes, box-row knobs, per-thread-store epilogue) out: the launches that
-// use none of them (every tap-mode launch; the stem is epilogue-bound and ran 16 % slower with the extra branches in
-// its epilogue, A/B on one GPU) get exactly the plain kernel.
-template <int MB, int BN, bool EXT>
+// Warp roles (384 threads = 3 warpgroups): warp 0 = TMA producer; warpgroups 1 and 2 = consumers.  Consumer g issues the
+// wgmma (M = 64) for rows [64 g, 64 g + 64) of every 128-row block of output channels, keeps those accumulators in
+// registers and writes them back through a swizzled staging block in smem and TMA stores.
+template <int MB>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 pw_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
                const __grid_constant__ CUtensorMap tmap_x4, const __grid_constant__ CUtensorMap tmap_y,
                const PwParams p) {
   constexpr int NB = BN / 64;
-  constexpr int ACC = (MB <= 2) ? 2 : 1;
-  static_assert(ACC * MB * BN <= TMEM_COLS, "TMEM budget");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int kchunks = (p.Cin + BK - 1) / BK;
-  const int ksteps_total = (p.Cin + 15) / 16;
   const int iters = p.taps * kchunks;      // K loop: (filter tap, 64-channel chunk)
   const int wres_bytes = p.wres ? iters * MB * A_BLK_BYTES : 0;
   const int stage_bytes = (p.wres ? 0 : MB * A_BLK_BYTES) + NB * B_BLK_BYTES;
@@ -178,26 +169,17 @@ pw_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
   uint8_t* outbuf = stage0 + p.stages * stage_bytes;
   uint64_t* full = reinterpret_cast<uint64_t*>(outbuf + p.out_bufs * OUT_BUF_BYTES);
   uint64_t* empty = full + MAX_STAGES;
-  uint64_t* tfull = empty + MAX_STAGES;
-  uint64_t* tempty = tfull + 2;
-  uint64_t* wfull = tempty + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wfull + 1);
+  uint64_t* wfull = empty + MAX_STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const bool x5 = EXT && p.x5, y5 = EXT && p.y5, epi_stg = EXT && p.epi_stg;
-  const int xbox = EXT ? p.xbox : BK, ybox = EXT ? p.ybox : 128;
+  const bool x5 = p.x5, y5 = p.y5;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < p.stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < ACC; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 128); }
+    for (int i = 0; i < p.stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }   // empty: one per consumer
     mbar_init(wfull, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     // ================= TMA producer =================
@@ -205,22 +187,19 @@ pw_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
       tma_prefetch_desc(&tmap_w);
       tma_prefetch_desc(&tmap_x);
       if (p.wres) {
-        // weights-stationary: the CTA keeps the (padded) filter rows of ITS group of output channels in smem for its
-        // whole life.  With several groups the grid is a multiple of num_mg, so tile t = it * grid + blockIdx.x
-        // always lands in group blockIdx.x % num_mg (t % num_mg below), and the CTAs of the other groups read the same
-        // activation tile at about the same time (L2 hits).
-        const int mg0 = blockIdx.x % p.num_mg;
+        // weights-stationary (one group of output channels): the CTA keeps the (padded) filter rows in smem for its
+        // whole life
         mbar_arrive_expect_tx(wfull, wres_bytes);
         for (int it = 0; it < iters; ++it)
 #pragma unroll
           for (int mb = 0; mb < MB; ++mb)
             tma_load_2d(wres + (it * MB + mb) * A_BLK_BYTES, &tmap_w, wfull, (it % kchunks) * BK,
-                        (it / kchunks) * p.Mpad + mg0 * (MB * 128) + mb * 128);
+                        (it / kchunks) * p.Mpad + mb * 128);
       }
       int s = 0, ph = 0;
-      for (int it = 0;; ++it) {
-        const int t = ((it / p.tgroup) * gridDim.x + blockIdx.x) * p.tgroup + it % p.tgroup;
-        if ((it / p.tgroup) * gridDim.x * p.tgroup >= p.num_tiles) break;
+      for (int tl = 0;; ++tl) {
+        const int t = ((tl / p.tgroup) * gridDim.x + blockIdx.x) * p.tgroup + tl % p.tgroup;
+        if ((tl / p.tgroup) * gridDim.x * p.tgroup >= p.num_tiles) break;
         if (t >= p.num_tiles) continue;
         const int mg = t % p.num_mg;
         const int tt = t / p.num_mg;
@@ -240,14 +219,9 @@ pw_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
           if (p.taps == 1) {
             if (x5) {
               tma_load_5d(st, &tmap_x, &full[s], 0, 0, p0 >> 6, kc * (BK / 8), n);
-            } else if (xbox == BK) {
+            } else {
 #pragma unroll
               for (int j = 0; j < NB; ++j) tma_load_3d(st + j * B_BLK_BYTES, &tmap_x, &full[s], p0 + j * 64, kc * BK, n);
-            } else {
-              for (int cg = 0; cg < BK; cg += xbox)
-#pragma unroll
-                for (int j = 0; j < NB; ++j)
-                  tma_load_3d(st + j * B_BLK_BYTES + cg * 128, &tmap_x, &full[s], p0 + j * 64, kc * BK + cg, n);
             }
           } else {
             // shifted window of this tap; out-of-image rows / columns are zero-filled by TMA (= zero padding)
@@ -263,155 +237,105 @@ pw_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      constexpr uint32_t IDESC = umma_idesc_bf16(128, BN, /*a_mn=*/0, /*b_mn=*/1);
-      if (p.wres) { mbar_wait(wfull, 0); tc_fence_after(); }
-      int s = 0, ph = 0, a = 0, aph = 0;
-      for (int it = 0;; ++it) {
-        const int t = ((it / p.tgroup) * gridDim.x + blockIdx.x) * p.tgroup + it % p.tgroup;
-        if ((it / p.tgroup) * gridDim.x * p.tgroup >= p.num_tiles) break;
-        if (t >= p.num_tiles) continue;
-        mbar_wait(&tempty[a], aph ^ 1);
-        tc_fence_after();
-        for (int it = 0; it < iters; ++it) {
-          const int kc = it % kchunks;
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint32_t st = smem_u32(stage0 + s * stage_bytes);
-          const uint32_t sa = p.wres ? smem_u32(wres + it * MB * A_BLK_BYTES) : st;
-          const uint32_t sb = p.wres ? st : st + MB * A_BLK_BYTES;
-          const int nsteps = min(4, ksteps_total - kc * 4);
-          for (int ks = 0; ks < nsteps; ++ks) {
-            // B: MN-major SW128. 16 channels = two 8-row groups (SBO = 1024 B); 64-px blocks at LBO = 8 KB
-            // (5-d box layout [8-ch group][px block][8 ch][128 B]: px blocks at LBO = 1 KB, channel groups at SBO = 2 KB)
-            const uint64_t bdesc = x5 ? umma_desc(sb + ks * (NB * 2048), 1024, NB * 1024)
-                                        : umma_desc(sb + ks * 2048, B_BLK_BYTES, 1024);
-#pragma unroll
-            for (int mb = 0; mb < MB; ++mb) {
-              // A: K-major SW128. 8-row groups at SBO = 1024 B; +32 B per 16-channel k-step
-              const uint64_t adesc = umma_desc(sa + mb * A_BLK_BYTES + ks * 32, 16, 1024);
-              umma_bf16(tmem_base + (a * MB + mb) * BN, adesc, bdesc, IDESC, (it | ks) ? 1u : 0u);
-            }
-          }
-          umma_commit(&empty[s]);
-          if (it == iters - 1) umma_commit(&tfull[a]);
-          if (++s == p.stages) { s = 0; ph ^= 1; }
-        }
-        if (++a == ACC) { a = 0; aph ^= 1; }
-      }
-    }
-  } else {
-    // ===== epilogue: TMEM -> registers -> swizzled smem -> TMA store of [128 ch][64 px] boxes =====
-    const int quarter = warp & 3;          // TMEM lane quarter this warp may access
-    const int row = quarter * 32 + lane;   // row of the 128-channel block (= TMEM lane)
-    const bool leader = (threadIdx.x == 64);
-    int a = 0, aph = 0, ob = 0;
-    for (int it = 0;; ++it) {
-      const int t = ((it / p.tgroup) * gridDim.x + blockIdx.x) * p.tgroup + it % p.tgroup;
-      if ((it / p.tgroup) * gridDim.x * p.tgroup >= p.num_tiles) break;
+  } else if (threadIdx.x >= 128) {
+    // ================= consumers: wgmma + epilogue =================
+    const int wg = (threadIdx.x >> 7) - 1;     // rows [64 wg, 64 wg + 64) of every 128-row block
+    const int w4 = (threadIdx.x >> 5) & 3;     // warp inside the warpgroup: fragment rows 16 w4 + lane / 4 (+ 8)
+    const bool wg_lead = (threadIdx.x & 127) == 0;
+    const bool leader = threadIdx.x == 128;    // issues the TMA stores
+    float acc[MB][BN / 2];
+    if (p.wres) mbar_wait(wfull, 0);
+    int s = 0, ph = 0, ob = 0;
+    for (int tl = 0;; ++tl) {
+      const int t = ((tl / p.tgroup) * gridDim.x + blockIdx.x) * p.tgroup + tl % p.tgroup;
+      if ((tl / p.tgroup) * gridDim.x * p.tgroup >= p.num_tiles) break;
       if (t >= p.num_tiles) continue;
       const int mg = t % p.num_mg;
       const int tt = t / p.num_mg;
       const int n = tt / p.tiles_per_image;
       const int p0 = (tt % p.tiles_per_image) * BN;
-      mbar_wait(&tfull[a], aph);
-      tc_fence_after();
-#pragma unroll 1
+      bool live[MB];                           // this warpgroup's 64 rows of block mb hold valid output channels
+#pragma unroll
+      for (int mb = 0; mb < MB; ++mb) live[mb] = mg * (MB * 128) + mb * 128 + 64 * wg < p.M;
+      int prev = -1;
+      for (int it = 0; it < iters; ++it) {
+        mbar_wait(&full[s], ph);
+        const uint32_t st = smem_u32(stage0 + s * stage_bytes);
+        const uint32_t sa = p.wres ? smem_u32(wres + it * MB * A_BLK_BYTES) : st;
+        const uint32_t sb = p.wres ? st : st + MB * A_BLK_BYTES;
+        // always 4 k-steps and every block: wgmma under a data-dependent branch is serialised by ptxas (C7520); the
+        // channels past Cin are zero in both operands (TMA zero fill, zero-padded weights), and so are the weight
+        // rows past M
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+          // B: MN-major SW128. 16 channels = two 8-row groups (SBO = 1024 B); 64-px blocks at LBO = 8 KB
+          // (5-d box layout [8-ch group][px block][8 ch][128 B]: px blocks at LBO = 1 KB, channel groups at SBO = 2 KB)
+          const uint64_t bdesc = x5 ? gmma_desc(sb + ks * (NB * 2048), 1024, NB * 1024)
+                                    : gmma_desc(sb + ks * 2048, B_BLK_BYTES, 1024);
+#pragma unroll
+          for (int mb = 0; mb < MB; ++mb) {
+            // A: K-major SW128. 8-row groups at SBO = 1024 B (this warpgroup's 64 rows start 8 KB in); +32 B per k-step
+            const uint64_t adesc = gmma_desc(sa + mb * A_BLK_BYTES + wg * 8192 + ks * 32, 16, 1024);
+            Wgmma<BN, 1>::mma(acc[mb], adesc, bdesc, (it | ks) ? 1u : 0u);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                         // the previous stage's MMAs are done reading it
+        if (prev >= 0 && wg_lead) mbar_arrive(&empty[prev]);
+        prev = s;
+        if (++s == p.stages) { s = 0; ph ^= 1; }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int mb = 0; mb < MB; ++mb) reg_fence(acc[mb]);
+      if (prev >= 0 && wg_lead) mbar_arrive(&empty[prev]);
+      // ===== epilogue: registers -> swizzled smem -> TMA store of [128 ch][64 px] boxes =====
+#pragma unroll
       for (int mb = 0; mb < MB; ++mb) {
         const int k0 = mg * (MB * 128) + mb * 128;
         if (k0 >= p.M) break;                       // block-uniform: nothing valid in this block
-        const int k = k0 + row;
-        const float bias = (k < p.M && p.bias) ? __bfloat162float(p.bias[k]) : 0.f;
-#pragma unroll 1
-        for (int h = 0; h < BN / 128; ++h) {        // 128 pixels (two 64-pixel blocks) of the tile at a time
-          const int ph0 = p0 + h * 128;
-          uint8_t* buf = outbuf + ob * OUT_BUF_BYTES;
-          if (epi_stg) {
-            // every thread has copied the previous contents of this buffer out (with two buffers the barrier of the
-            // block in between already guarantees that)
-            if (p.out_bufs == 1) named_bar_sync(1, 128);
-          } else {
-            // the TMA store that last read this buffer must have finished reading it
-            if (leader) { if (p.out_bufs == 2) tma_store_wait_read<1>(); else tma_store_wait_read<0>(); }
-            named_bar_sync(1, 128);
-          }
+        uint8_t* buf = outbuf + ob * OUT_BUF_BYTES;
+        // the TMA store that last read this buffer must have finished reading it
+        if (leader) { if (p.out_bufs == 2) tma_store_wait_read<1>(); else tma_store_wait_read<0>(); }
+        named_bar_sync(1, 256);
+        if (live[mb]) {
+          const int r0 = 64 * wg + 16 * w4 + (lane >> 2);   // fragment rows r0 and r0 + 8 of the block
 #pragma unroll
-          for (int cc = 0; cc < 4; ++cc) {
-            uint32_t r[32];
-            tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (a * MB + mb) * BN + h * 128 + cc * 32, r);
-            tmem_ld_wait();
-            uint8_t* blk = y5 ? buf + (row >> 3) * 2048 + (cc >> 1) * 1024 + (row & 7) * 128
-                                : buf + (cc >> 1) * (128 * 128) + row * 128;
+          for (int h = 0; h < 2; ++h) {
+            const int r = r0 + 8 * h;
+            const int k = k0 + r;
+            const float bias = (k < p.M && p.bias) ? __bfloat162float(p.bias[k]) : 0.f;
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              uint4 v;
-              v.x = pack_bf16x2(__uint_as_float(r[8 * q + 0]) + bias, __uint_as_float(r[8 * q + 1]) + bias);
-              v.y = pack_bf16x2(__uint_as_float(r[8 * q + 2]) + bias, __uint_as_float(r[8 * q + 3]) + bias);
-              v.z = pack_bf16x2(__uint_as_float(r[8 * q + 4]) + bias, __uint_as_float(r[8 * q + 5]) + bias);
-              v.w = pack_bf16x2(__uint_as_float(r[8 * q + 6]) + bias, __uint_as_float(r[8 * q + 7]) + bias);
-              const int chunk = ((cc & 1) * 4 + q) ^ (row & 7);   // SWIZZLE_128B: 16-B chunk ^ (row % 8)
-              *reinterpret_cast<uint4*>(blk + chunk * 16) = v;
+            for (int q = 0; q < BN / 8; ++q) {          // 8-pixel column group q: pixels 8q + 2 (lane % 4) + {0, 1}
+              const int j = q >> 3;                     // 64-pixel block
+              uint8_t* rowp = y5 ? buf + (r >> 3) * 2048 + j * 1024 + (r & 7) * 128 : buf + j * (128 * 128) + r * 128;
+              const uint32_t v = pack_bf16x2(acc[mb][4 * q + 2 * h] + bias, acc[mb][4 * q + 2 * h + 1] + bias);
+              // SWIZZLE_128B: 16-B chunk ^ (row % 8)
+              *reinterpret_cast<uint32_t*>(rowp + (((q & 7) ^ (r & 7)) << 4) + (lane & 3) * 4) = v;
             }
           }
-          if (h == BN / 128 - 1 && (mb == MB - 1 || k0 + 128 >= p.M)) {   // last read of this tile's accumulators
-            tc_fence_before();
-            mbar_arrive(&tempty[a]);
-          }
-          if (epi_stg) {
-            // staged [128 ch][2 x 64 px] tile -> global: 8 consecutive threads write one full 128-B line of a channel
-            // row, so every store instruction of a warp fills 4 whole lines.  Nothing waits for the writes to land:
-            // the staging buffer is free again as soon as it has been read, and the TMA unit only serves the loads.
-            named_bar_sync(1, 128);
-            const int et = threadIdx.x - 64, g = et & 7, r0 = et >> 3;
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-              const int px = ph0 + j * 64 + g * 8;
-              if (px < p.P) {
-#pragma unroll
-                for (int rr = 0; rr < 8; ++rr) {
-                  const int rw = rr * 16 + r0;
-                  if (k0 + rw < p.M) {
-                    const uint4 v = *reinterpret_cast<const uint4*>(buf + j * (128 * 128) + rw * 128 + ((g ^ (rw & 7)) << 4));
-                    __stcs(reinterpret_cast<uint4*>(p.y + ((size_t)n * p.M + k0 + rw) * p.P + px), v);
-                  }
-                }
-              }
-            }
-          } else {
-            fence_proxy_async();        // make the smem writes visible to the TMA (async proxy)
-            named_bar_sync(1, 128);
-            if (leader) {
-              if (y5) {
-                tma_store_5d(&tmap_y, buf, 0, 0, ph0 >> 6, k0 >> 3, n);
-              } else if (ybox == 128) {
-#pragma unroll
-                for (int j = 0; j < 2; ++j) tma_store_3d(&tmap_y, buf + j * (128 * 128), ph0 + j * 64, k0, n);
-              } else {
-                for (int cg = 0; cg < 128 && k0 + cg < p.M; cg += ybox)
-#pragma unroll
-                  for (int j = 0; j < 2; ++j)
-                    tma_store_3d(&tmap_y, buf + j * (128 * 128) + cg * 128, ph0 + j * 64, k0 + cg, n);
-              }
-              tma_store_commit();
-            }
-          }
-          if (p.out_bufs == 2) ob ^= 1;
         }
+        fence_proxy_async();        // make the smem writes visible to the TMA (async proxy)
+        named_bar_sync(1, 256);
+        if (leader) {
+          if (y5) {
+            tma_store_5d(&tmap_y, buf, 0, 0, p0 >> 6, k0 >> 3, n);
+          } else {
+#pragma unroll
+            for (int j = 0; j < 2; ++j) tma_store_3d(&tmap_y, buf + j * (128 * 128), p0 + j * 64, k0, n);
+          }
+          tma_store_commit();
+        }
+        if (p.out_bufs == 2) ob ^= 1;
       }
-      if (++a == ACC) { a = 0; aph ^= 1; }
     }
-    if (leader && !epi_stg) tma_store_wait_read<0>();
+    if (leader) tma_store_wait_read<0>();
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
-// tuning knob: positive integer from the environment, else `dflt` (tools/wgrad_probe.py sweeps these)
+// tuning knob: positive integer from the environment, else `dflt`
 // Every knob is read from the environment ONCE per process (getenv on the launch path showed up in the
 // N=8 step, which is CPU-bound): a small table keyed by the name's address (names are string literals).
 struct EnvKnob { const char* name; const char* val; };
@@ -434,40 +358,34 @@ inline int sm_count() {
   if (!sms) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
   }
   return sms;
 }
 
-constexpr int SMEM_LIMIT = 222 * 1024;   // leave room for a small co-resident kernel (halo post/collect, boundary strips)
+constexpr int SMEM_LIMIT = 222 * 1024;   // of H100's 227 KB per block: room for a small co-resident kernel (halo post/collect)
 constexpr int SMEM_AUX = 1024 /*align*/ + 512 /*barriers*/;
 
-template <int MB, int BN, bool EXT>
-int launch_pw_ext(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& tx4, const CUtensorMap& ty, PwParams p,
+template <int MB>
+int launch_pw(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& tx4, const CUtensorMap& ty, PwParams p,
               cudaStream_t st) {
   const int kchunks = (p.Cin + BK - 1) / BK;
   const int budget = SMEM_LIMIT - SMEM_AUX;
   const int wres_bytes = p.taps * kchunks * MB * A_BLK_BYTES;
   const int sms = sm_count();
-  int grid = p.num_tiles < sms ? p.num_tiles : sms;
+  const int grid = p.num_tiles < sms ? p.num_tiles : sms;
   if (p.num_tiles < 16 * sms) p.tgroup = 1;   // small problems: keep every SM busy
-  // stationary weights with several groups of output channels: every CTA serves one group (see the kernel), which needs
-  // a grid that is a multiple of num_mg and tiles dealt round-robin
-  bool stationary = wres_bytes <= 128 * 1024;
-  if (stationary && p.num_mg > 1) {
-    if (p.stationary_ok && grid >= 4 * p.num_mg) { grid = grid / p.num_mg * p.num_mg; p.tgroup = 1; }
-    else stationary = false;
-  }
-  p.wres = stationary ? 1 : 0;
+  // stationary weights: only with one group of output channels (every CTA then needs the same filter rows)
+  p.wres = (wres_bytes <= 128 * 1024 && p.num_mg == 1) ? 1 : 0;
   const int stage_bytes = (p.wres ? 0 : MB * A_BLK_BYTES) + (BN / 64) * B_BLK_BYTES;
   const int rem = budget - (p.wres ? wres_bytes : 0);
   p.out_bufs = 2;
   p.stages = (rem - 2 * OUT_BUF_BYTES) / stage_bytes;
-  if (p.stages < 3 || env_int("SPC_PW_OUTBUFS", 2) == 1) { p.out_bufs = 1; p.stages = (rem - OUT_BUF_BYTES) / stage_bytes; }
+  if (p.stages < 3) { p.out_bufs = 1; p.stages = (rem - OUT_BUF_BYTES) / stage_bytes; }
   if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
-  SPC_REQUIRE(p.stages >= 2, "tcgen05 conv: shared memory budget too small (MB=%d kchunks=%d)", MB, kchunks);
+  SPC_REQUIRE(p.stages >= 2, "wgmma conv: shared memory budget too small (MB=%d kchunks=%d)", MB, kchunks);
   const int smem = (p.wres ? wres_bytes : 0) + p.stages * stage_bytes + p.out_bufs * OUT_BUF_BYTES + SMEM_AUX;
-  auto kern = pw_gemm_kernel<MB, BN, EXT>;
+  auto kern = pw_gemm_kernel<MB>;
   static bool attr_set = false;   // per instantiation
   if (!attr_set) {
     SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
@@ -477,13 +395,6 @@ int launch_pw_ext(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMa
   count_launch();
   SPC_CHECK_CUDA(cudaGetLastError());
   return SPC_OK;
-}
-
-template <int MB, int BN>
-int launch_pw(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& tx4, const CUtensorMap& ty, const PwParams& p,
-              cudaStream_t st) {
-  const bool ext = p.x5 || p.y5 || p.epi_stg || p.xbox != BK || p.ybox != 128;
-  return ext ? launch_pw_ext<MB, BN, true>(tw, tx, tx4, ty, p, st) : launch_pw_ext<MB, BN, false>(tw, tx, tx4, ty, p, st);
 }
 
 int make_act_tmap(CUtensorMap* m, const void* base, int P, int Cc, int N, int box_rows) {
@@ -504,7 +415,7 @@ int make_act_tmap5(CUtensorMap* m, const void* base, int P, int Cc, int N, int g
 
 int launch_shift_copies(const void* x, void* xs, size_t planes, int H, int W, int S, int pw, int cs, cudaStream_t st);
 
-// Geometry of one tcgen05 convolution launch (fprop, or dgrad expressed as a convolution of dY).
+// Geometry of one wgmma convolution launch (fprop, or dgrad expressed as a convolution of dY).
 struct TcConv {
   const __nv_bfloat16* w;      // original filter [K][C][R][S]
   long long sm, sc;            // strides of (output channel m, reduction channel c) in w
@@ -532,7 +443,7 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
   const uintptr_t xs_addr = (wp_addr + wp_bytes + 1023) & ~(uintptr_t)1023;
   const size_t xs_bytes = copies ? (size_t)c.S * c.N * c.Cin * c.H * Wo * 2 : 0;
   const size_t need = (xs_addr - ws0) + xs_bytes;
-  SPC_REQUIRE((ws && ws_bytes >= need) || need <= 1024, "tcgen05 conv: workspace too small (%zu < %zu)", ws_bytes, need);
+  SPC_REQUIRE((ws && ws_bytes >= need) || need <= 1024, "wgmma conv: workspace too small (%zu < %zu)", ws_bytes, need);
   const __nv_bfloat16* wp = c.prepacked;
   if (!c.prepacked) {
     __nv_bfloat16* wpm = reinterpret_cast<__nv_bfloat16*>(wp_addr);
@@ -554,27 +465,12 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
     xsrc = reinterpret_cast<const __nv_bfloat16*>(xs);
   }
   CUtensorMap tw, tx, tx4, ty;
-  // Wide-N variant (256-pixel tiles, one 128-row block of output channels per CTA with its filter rows resident in
-  // shared memory, double-buffered accumulators): for pointwise layers with 3+ blocks of output channels and 256..512
-  // input channels, which are bound by the tensor pipe -- a 128x128x16 MMA costs almost what a 128x256x16 one does
-  // (measured 185-270 vs 222 clk), so N = 256 should nearly halve the MMA time per pixel.  MEASURED (profiles/
-  // r2h_pw_n256.txt): slower, 416->416 @1024^2 0.56 -> 0.65 ms -- with the filter rows resident only two 32 KB
-  // activation stages fit, and 64 KB in flight per SM at ~2 us of load latency caps the CTA at ~35 GB/s.  Kept behind
-  // SPC_PW_N256=1 (off by default); results are bit-identical to the default path.
-  const char* n256_env = env_get("SPC_PW_N256");
-  const bool n256 = taps == 1 && cs == 1 && Mpad / 128 >= 3 && (Cpad / BK) * A_BLK_BYTES <= 128 * 1024 && P % 256 == 0 &&
-                    (n256_env ? atoi(n256_env) != 0 : false);
-  const int BN = n256 ? 256 : BN_DEFAULT;
-  int xbox = (taps == 1) ? env_int("SPC_PW_XBOX", BK) : BK, ybox = env_int("SPC_PW_YBOX", 128);
-  if (xbox != 8 && xbox != 16 && xbox != 32) xbox = BK;
-  if (ybox != 8 && ybox != 16 && ybox != 32 && ybox != 64) ybox = 128;
-  // 5-d boxes (see PwParams::x5): measured on B200 (profiles/r2f_pw_box5.txt) +20..32 % on the layers whose channel
-  // planes span several 2 MB pages (104->208 @4096^2: 4.30 -> 5.67 TB/s), neutral at 1024^2 planes -> on from 4 MB planes.
+  // 5-d boxes (see PwParams::x5) for the layers whose channel planes span several 2 MB pages (from 4 MB planes).
   // SPC_PW_BOX5 = 0..3 overrides (bit 0: activations, bit 1: outputs).
   const char* box5_env = env_get("SPC_PW_BOX5");
   const int box5 = box5_env ? atoi(box5_env) : ((size_t)P * 2 >= ((size_t)4 << 20) ? 3 : 0);
-  const int x5 = (taps == 1 && cs == 1 && (box5 & 1) && P % 64 == 0 && c.Cin % 8 == 0 && xbox == BK) ? 1 : 0;
-  const int y5 = (taps == 1 && (box5 & 2) && P % 64 == 0 && c.M % 8 == 0 && ybox == 128) ? 1 : 0;
+  const int x5 = (taps == 1 && cs == 1 && (box5 & 1) && P % 64 == 0 && c.Cin % 8 == 0) ? 1 : 0;
+  const int y5 = (taps == 1 && (box5 & 2) && P % 64 == 0 && c.M % 8 == 0) ? 1 : 0;
   {
     const uint64_t dims[2] = {(uint64_t)Cpad, (uint64_t)taps * Mpad};
     const uint64_t strides[2] = {0, (uint64_t)Cpad * 2};
@@ -592,52 +488,30 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
     if (rc) return rc;
     tx = tx4;
   } else {
-    rc = x5 ? make_act_tmap5(&tx, x, Pin, c.Cin, c.N, BK / 8, BN / 64) : make_act_tmap(&tx, x, Pin, c.Cin, c.N, xbox);
+    rc = x5 ? make_act_tmap5(&tx, x, Pin, c.Cin, c.N, BK / 8, BN / 64) : make_act_tmap(&tx, x, Pin, c.Cin, c.N, BK);
     if (rc) return rc;
     tx4 = tx;
   }
-  rc = y5 ? make_act_tmap5(&ty, y, P, c.M, c.N, 16, 2) : make_act_tmap(&ty, y, P, c.M, c.N, ybox);
+  rc = y5 ? make_act_tmap5(&ty, y, P, c.M, c.N, 16, 2) : make_act_tmap(&ty, y, P, c.M, c.N, 128);
   if (rc) return rc;
   PwParams p{};
-  p.xbox = xbox; p.ybox = ybox; p.x5 = x5; p.y5 = y5;
+  p.x5 = x5; p.y5 = y5;
   p.bias = bias; p.M = c.M; p.Cin = c.Cin; p.P = P; p.N = c.N;
   p.taps = taps; p.S = c.S; p.ph = c.ph; p.pw = c.pw; p.W = Wo; p.Mpad = Mpad;
   p.shiftN = copies ? c.N : 0;
   p.rowmul = cs;
-  p.y = y;
-  p.epi_stg = (env_int("SPC_PW_EPI_STG", 0) == 1 && P % 8 == 0 && !y5) ? 1 : 0;
   {
     const char* e = env_get("SPC_TILE_GROUP");
-    p.tgroup = e ? atoi(e) : 1;   // measured: no effect on B200 (tools/stride_probe.py), kept as a knob
+    p.tgroup = e ? atoi(e) : 1;
     if (p.tgroup < 1) p.tgroup = 1;
   }
+  // groups of at most two 128-row blocks of output channels: a consumer thread holds 64 fp32 accumulators per block
   const int MBtot = Mpad / 128;
-  // 3+ blocks of output channels: two groups of 256 with double-buffered accumulators (the epilogue of
-  // one tile overlaps the K loop of the next) beat one group of 512 whose single accumulator set
-  // serialises them, even though the activation tile is then read once per group (from L2).
-  // Measured (r1, profiles/): wins for Cin <= 416 (+6..19 %), loses for Cin >= 624 where the K loop is
-  // long enough to hide the epilogue and the extra activation reads cost more than the overlap gains.
-  int mb = MBtot >= 3 ? (c.Cin <= 512 ? 2 : 4) : MBtot;
-  // Stationary weights with several groups of output channels on 128-pixel tiles (SPC_PW_STATIONARY=1, off by default):
-  // measured SLOWER than streaming them (416->416 @1024^2: 0.56 -> 0.83 ms, profiles/r2h_pw_stationary.txt) -- with
-  // one block per CTA the tensor pipe issues half as many MACs per MMA slot.  The wide-N variant above is the one
-  // that pays.
-  {
-    const char* se = env_get("SPC_PW_STATIONARY");
-    const int kch = (c.Cin + BK - 1) / BK;
-    p.stationary_ok = ((se && atoi(se) != 0) || n256) && taps * kch * A_BLK_BYTES <= 128 * 1024;
-    if (p.stationary_ok && MBtot >= 3 && !n256) mb = (taps * kch * 2 * A_BLK_BYTES <= 128 * 1024) ? 2 : 1;
-    if (n256) mb = 1;
-  }
-  if (MBtot >= 3 && !n256 && env_get("SPC_PW_MB4")) mb = 4;                 // A/B knobs
-  if (MBtot >= 3 && !n256 && env_get("SPC_PW_MB2")) mb = 2;
+  const int mb = MBtot >= 2 ? 2 : 1;
   p.num_mg = (MBtot + mb - 1) / mb;
   p.tiles_per_image = (P + BN - 1) / BN;
   p.num_tiles = p.tiles_per_image * c.N * p.num_mg;
-  if (n256) return launch_pw<1, 256>(tw, tx, tx4, ty, p, st);
-  if (mb == 1) return launch_pw<1, 128>(tw, tx, tx4, ty, p, st);
-  if (mb == 2) return launch_pw<2, 128>(tw, tx, tx4, ty, p, st);
-  return launch_pw<4, 128>(tw, tx, tx4, ty, p, st);
+  return mb == 2 ? launch_pw<2>(tw, tx, tx4, ty, p, st) : launch_pw<1>(tw, tx, tx4, ty, p, st);
 }
 
 // pointwise helper (1x1): Y[N][M][P] = Wp[M x Cin] * X[N][Cin][P]
@@ -652,15 +526,21 @@ int run_pw(const __nv_bfloat16* w, int ld, int transpose, int M, int Cin, const 
 
 // ---- wgrad kernel: dW[K x C x taps] += dY[K x P] * shift_tap(X)[C x P]^T -------------------------
 // Both operands are K-major straight from NCHW (pixels = reduction dim, contiguous).  One work
-// item = (group of MG 128-row blocks of dY, one block of nblk input channels, a pass of TG filter
+// item = (group of MG 128-row blocks of dY, one block of NBLK input channels, a pass of TG filter
 // taps, a split of the pixel range); accumulators for all (tap, m-block) pairs of the item live in
-// TMEM ((TG*MG) x nblk columns <= 512) and are flushed with fp32 atomics.
+// registers (NA = TG * MG <= WG_ACC / NBLK blocks of [64 rows x NBLK] per consumer thread set) and are flushed with fp32
+// atomics.  NA is a template parameter and every k-step issues all NA MMAs: wgmma under a data-dependent branch is
+// serialised by ptxas (C7520).  The last tap pass of a filter may use fewer than TG taps; the accumulators of its
+// missing taps read stale tap slots of the stage and are never flushed.
+constexpr int WG_ACC = 256;   // accumulator columns per consumer warpgroup: 128 fp32 registers per thread
+
 struct WgParams {
   float* dw;        // [K][C][taps] fp32 (atomic accumulation)
   int K, C, P, N;
-  int nblk;         // columns (input channels) per accumulator block, multiple of 16, <= 256
+  int nblk;         // columns (input channels) per accumulator block: the kernel's NBLK
   int n_blocks;     // ceil(C / nblk)
-  int mgroups;      // ceil(ceil(K/128) / MG)
+  int MG;           // 128-row blocks of dY per item
+  int mgroups;      // ceil(ceil(K/mrows) / MG)
   int splits;       // pixel-range splits per item
   int chunks_total; // N * ceil(P/64)
   int chunks_per_image;
@@ -669,7 +549,7 @@ struct WgParams {
   int TG, passes;   // taps per pass, ceil(taps / TG)
   int W, shiftN;    // OUTPUT image width; N if x is the S column-shifted copies, else 0
   int rowmul;       // input row = rowmul * output row + tap row offset
-  int mrows;        // dY rows per 128-lane block (<= 128): K split EVENLY over its blocks, so every item streams the
+  int mrows;        // dY rows per 128-row block (<= 128): K split EVENLY over its blocks, so every item streams the
                     // same number of valid rows and the CTAs that share an x chunk stay in lock-step (L2 hits)
   int split_major;  // 1: concurrently running CTAs cover all (m-group, channel-block, pass) groups of the SAME
                     //    pixel range, so the dY / x chunks every group re-reads come from L2, not HBM
@@ -677,33 +557,26 @@ struct WgParams {
   int dy5, x5;      // wide stages: operand moves as one 5-d box [8-ch group][px block][8 ch][128 B] (see PwParams::x5)
 };
 
-template <int MG>
+template <int NBLK, int NA>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x,
                 const __grid_constant__ CUtensorMap tmap_x4, const WgParams p) {
+  static_assert(NA * NBLK <= WG_ACC, "accumulator registers");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int b_bytes = p.nblk * 128;                        // one tap's [nblk ch][64 px] box
+  const int MG = p.MG;
+  const int b_bytes = NBLK * 128;                          // one tap's [NBLK ch][64 px] box
   const int b_slot = (b_bytes + 1023) & ~1023;
   const int stage_bytes = p.pb * (MG * A_BLK_BYTES + p.TG * b_slot);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
   uint64_t* empty = full + MAX_STAGES;
-  uint64_t* tfull = empty + MAX_STAGES;
-  uint64_t* tempty = tfull + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < p.stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    mbar_init(tfull, 1);
-    mbar_init(tempty, 128);
+    for (int i = 0; i < p.stages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }   // empty: one per consumer
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int ngroups = p.mgroups * p.n_blocks * p.passes;
   const int num_items = ngroups * p.splits;
   const int per_split = (p.chunks_total + p.splits - 1) / p.splits;
@@ -726,14 +599,12 @@ pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_consta
       int s = 0, ph = 0;
       for (int it = blockIdx.x; it < num_items; it += gridDim.x) {
         WG_DECODE(it)
-        (void)mgp;
         for (int ch = c_begin; ch < c_end; ++ch) {
           const int n = ch / p.chunks_per_image, p0 = (ch % p.chunks_per_image) * (64 * p.pb);
           mbar_wait(&empty[s], ph ^ 1);
           uint8_t* st = smem + s * stage_bytes;
           mbar_arrive_expect_tx(&full[s], p.pb * (MG * p.mrows * 128 + ntap * b_bytes));
           if (p.pb == 2) {   // wide stage (taps == 1): two 64-pixel blocks of every operand row
-#pragma unroll
             for (int i = 0; i < MG; ++i) {
               uint8_t* da = st + i * (2 * A_BLK_BYTES);
               const int r0 = (mgp * MG + i) * p.mrows;
@@ -746,47 +617,50 @@ pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_consta
             }
             uint8_t* xa = st + MG * (2 * A_BLK_BYTES);
             if (p.x5) {
-              tma_load_5d(xa, &tmap_x, &full[s], 0, 0, p0 >> 6, (nb * p.nblk) >> 3, n);
+              tma_load_5d(xa, &tmap_x, &full[s], 0, 0, p0 >> 6, (nb * NBLK) >> 3, n);
             } else {
-              tma_load_3d(xa, &tmap_x, &full[s], p0, nb * p.nblk, n);
-              tma_load_3d(xa + b_slot, &tmap_x, &full[s], p0 + 64, nb * p.nblk, n);
+              tma_load_3d(xa, &tmap_x, &full[s], p0, nb * NBLK, n);
+              tma_load_3d(xa + b_slot, &tmap_x, &full[s], p0 + 64, nb * NBLK, n);
             }
             if (++s == p.stages) { s = 0; ph ^= 1; }
             continue;
           }
-#pragma unroll
           for (int i = 0; i < MG; ++i)
             tma_load_3d(st + i * A_BLK_BYTES, &tmap_dy, &full[s], p0, (mgp * MG + i) * p.mrows, n);
           if (p.taps == 1) {
-            tma_load_3d(st + MG * A_BLK_BYTES, &tmap_x, &full[s], p0, nb * p.nblk, n);
+            tma_load_3d(st + MG * A_BLK_BYTES, &tmap_x, &full[s], p0, nb * NBLK, n);
           } else {
             const int hq = p0 / p.W, wq = p0 - hq * p.W;
             for (int t = 0; t < ntap; ++t) {
               const int tap = tap0 + t;
               tma_load_4d(st + MG * A_BLK_BYTES + t * b_slot, &tmap_x4, &full[s], wq, hq * p.rowmul + tap / p.S - p.ph,
-                          nb * p.nblk, n + (tap % p.S) * p.shiftN);
+                          nb * NBLK, n + (tap % p.S) * p.shiftN);
             }
           }
           if (++s == p.stages) { s = 0; ph ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_bf16(128, p.nblk, 0, 0);
-      int s = 0, ph = 0, aph = 0;
-      for (int it = blockIdx.x; it < num_items; it += gridDim.x) {
-        WG_DECODE(it)
-        (void)nb; (void)mgp;
-        mbar_wait(tempty, aph ^ 1);
-        tc_fence_after();
-        for (int ch = c_begin; ch < c_end; ++ch) {
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * stage_bytes);
+  } else if (threadIdx.x >= 128) {
+    // ================= consumers: wgmma over rows [64 wg, 64 wg + 64) of every dY block, then the flush =================
+    const int wg = (threadIdx.x >> 7) - 1;
+    const int w4 = (threadIdx.x >> 5) & 3;
+    const bool wg_lead = (threadIdx.x & 127) == 0;
+    const bool live = 64 * wg < p.mrows;       // rows >= mrows of a block are not dY rows of this block
+    float acc[NA][NBLK / 2];
+    int s = 0, ph = 0;
+    for (int it = blockIdx.x; it < num_items; it += gridDim.x) {
+      WG_DECODE(it)
+      const int nacc = ntap * MG;              // accumulator a = (tap a / MG, dY block a % MG); a >= nacc: not flushed
+      int prev = -1;
+      for (int ch = c_begin; ch < c_end; ++ch) {
+        mbar_wait(&full[s], ph);
+        const uint32_t sa = smem_u32(smem + s * stage_bytes);
+        wgmma_fence();
+        {
           if (p.pb == 2) {
             // wide stage: pixel block j of a 5-d box sits 1 KB after block 0 inside every 2 KB channel group; of a pair
-            // of 3-d boxes, one whole box later
+            // of 3-d boxes, one whole box later.  This warpgroup's 64 rows start 8 row groups (8 SBO) in.
             const uint32_t sb = sa + MG * (2 * A_BLK_BYTES);
             const uint32_t aj = p.dy5 ? 1024 : A_BLK_BYTES, asbo = p.dy5 ? 2048 : 1024;
             const uint32_t bj = p.x5 ? 1024 : b_slot, bsbo = p.x5 ? 2048 : 1024;
@@ -794,126 +668,108 @@ pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_consta
             for (int j = 0; j < 2; ++j) {
 #pragma unroll
               for (int ks = 0; ks < 4; ++ks) {
-                const uint64_t bdesc = umma_desc(sb + j * bj + ks * 32, 16, bsbo);
+                const uint64_t bdesc = gmma_desc(sb + j * bj + ks * 32, 16, bsbo);
 #pragma unroll
-                for (int i = 0; i < MG; ++i) {
-                  const uint64_t adesc = umma_desc(sa + i * (2 * A_BLK_BYTES) + j * aj + ks * 32, 16, asbo);
-                  umma_bf16(tmem_base + i * p.nblk, adesc, bdesc, idesc, (ch > c_begin || ks > 0 || j > 0) ? 1u : 0u);
+                for (int a = 0; a < NA; ++a) {   // wide stages only with taps == 1: NA == MG
+                  const uint64_t adesc = gmma_desc(sa + a * (2 * A_BLK_BYTES) + wg * 8 * asbo + j * aj + ks * 32, 16, asbo);
+                  Wgmma<NBLK, 0>::mma(acc[a], adesc, bdesc, (ch > c_begin || ks > 0 || j > 0) ? 1u : 0u);
                 }
               }
             }
-            umma_commit(&empty[s]);
-            if (++s == p.stages) { s = 0; ph ^= 1; }
-            continue;
-          }
-          const uint32_t sb = sa + MG * A_BLK_BYTES;
-          for (int t = 0; t < ntap; ++t) {
+          } else {
+            const uint32_t sb = sa + MG * A_BLK_BYTES;
 #pragma unroll
             for (int ks = 0; ks < 4; ++ks) {
-              const uint64_t bdesc = umma_desc(sb + t * b_slot + ks * 32, 16, 1024);
 #pragma unroll
-              for (int i = 0; i < MG; ++i) {
-                const uint64_t adesc = umma_desc(sa + i * A_BLK_BYTES + ks * 32, 16, 1024);
-                umma_bf16(tmem_base + (t * MG + i) * p.nblk, adesc, bdesc, idesc, (ch > c_begin || ks > 0) ? 1u : 0u);
+              for (int a = 0; a < NA; ++a) {
+                const int t = a / MG, i = a - t * MG;
+                const uint64_t bdesc = gmma_desc(sb + t * b_slot + ks * 32, 16, 1024);
+                const uint64_t adesc = gmma_desc(sa + i * A_BLK_BYTES + wg * 8192 + ks * 32, 16, 1024);
+                Wgmma<NBLK, 0>::mma(acc[a], adesc, bdesc, (ch > c_begin || ks > 0) ? 1u : 0u);
               }
             }
           }
-          umma_commit(&empty[s]);
-          if (++s == p.stages) { s = 0; ph ^= 1; }
         }
-        umma_commit(tfull);
-        aph ^= 1;
+        wgmma_commit();
+        wgmma_wait<1>();                         // the previous stage's MMAs are done reading it
+        if (prev >= 0 && wg_lead) mbar_arrive(&empty[prev]);
+        prev = s;
+        if (++s == p.stages) { s = 0; ph ^= 1; }
       }
-    }
-  } else {
-    const int quarter = warp & 3;
-    int aph = 0;
-    for (int it = blockIdx.x; it < num_items; it += gridDim.x) {
-      WG_DECODE(it)
-      mbar_wait(tfull, aph);
-      tc_fence_after();
-      if (c_end > c_begin) {
-#pragma unroll 1
-        for (int t = 0; t < ntap; ++t) {
-#pragma unroll 1
-          for (int i = 0; i < MG; ++i) {
-            const int rib = quarter * 32 + lane;                     // row inside the block (= TMEM lane)
-            const int k = rib < p.mrows ? (mgp * MG + i) * p.mrows + rib : p.K;   // lanes >= mrows hold garbage
-#pragma unroll 1
-            for (int cc = 0; cc * 32 < p.nblk; ++cc) {
-              uint32_t r[32];
-              tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (t * MG + i) * p.nblk + cc * 32, r);
-              tmem_ld_wait();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int a = 0; a < NA; ++a) reg_fence(acc[a]);
+      if (prev >= 0 && wg_lead) mbar_arrive(&empty[prev]);
+      if (c_end > c_begin && live) {
+#pragma unroll
+        for (int a = 0; a < NA; ++a) {
+          if (a < nacc) {
+            const int t = a / MG, i = a - t * MG;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int rib = 64 * wg + 16 * w4 + (lane >> 2) + 8 * h;   // row inside the block
+              const int k = rib < p.mrows ? (mgp * MG + i) * p.mrows + rib : p.K;
               if (k < p.K) {
 #pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                  const int cl = cc * 32 + j;
-                  const int c = nb * p.nblk + cl;
-                  if (cl < p.nblk && c < p.C)
-                    atomicAdd(&p.dw[((size_t)k * p.C + c) * p.taps + tap0 + t], __uint_as_float(r[j]));
+                for (int q = 0; q < NBLK / 8; ++q) {
+#pragma unroll
+                  for (int e = 0; e < 2; ++e) {
+                    const int c = nb * NBLK + 8 * q + 2 * (lane & 3) + e;
+                    if (c < p.C) atomicAdd(&p.dw[((size_t)k * p.C + c) * p.taps + tap0 + t], acc[a][4 * q + 2 * h + e]);
+                  }
                 }
               }
             }
           }
         }
       }
-      tc_fence_before();
-      mbar_arrive(tempty);
-      aph ^= 1;
     }
   }
 #undef WG_DECODE
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
-template <int MG>
+template <int NBLK, int NA>
 int launch_wg(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMap& tx4, WgParams p, cudaStream_t st) {
-  const int b_slot = (p.nblk * 128 + 1023) & ~1023;
-  // taps per pass: TMEM columns and a stage small enough for >= 2 pipeline stages
-  int TG = 512 / (MG * p.nblk);
-  if (TG > p.taps) TG = p.taps;
-  while (TG > 1 && MG * A_BLK_BYTES + TG * b_slot > (SMEM_LIMIT - SMEM_AUX) / 2) --TG;
+  const int b_slot = (NBLK * 128 + 1023) & ~1023;
+  const int TG = NA / p.MG;                // taps per pass (chosen by launch_wg_na)
   p.TG = TG;
   p.passes = (p.taps + TG - 1) / TG;
-  const int stage_bytes = p.pb * (MG * A_BLK_BYTES + TG * b_slot);
+  const int stage_bytes = p.pb * (p.MG * A_BLK_BYTES + TG * b_slot);
   p.stages = (SMEM_LIMIT - SMEM_AUX) / stage_bytes;
   if (p.stages > 6) p.stages = 6;
   p.stages = min(p.stages, env_int("SPC_WG_STAGES", p.stages));
-  SPC_REQUIRE(p.stages >= 2, "tcgen05 wgrad: smem budget");
+  SPC_REQUIRE(p.stages >= 2, "wgmma wgrad: smem budget");
   const int sms = sm_count();
   const int groups = p.mgroups * p.n_blocks * p.passes;
   // items = groups * splits on a persistent grid of `sms` CTAs.  Every item ends by adding its accumulators to dw with
-  // fp32 atomics, and that flush is a CHIP-WIDE cost (~90 G atomics/s measured, profiles/r2_wgrad_splits.txt): with
-  // few pixels per item it dominates (104->416 on a 1024x128 tile: 0.159 ms at 296 items, 0.082 at 74).  Pick the
-  // split count that minimises   waves * chunks_per_item * t_chunk + items * elems_per_item / 90e9,
-  // t_chunk = the slower of the item's MMA chain and its operand bytes at the per-SM share of L2 bandwidth.
+  // fp32 atomics, and that flush is a chip-wide cost: with few pixels per item it dominates.  Pick the split count
+  // that minimises   waves * chunks_per_item * t_chunk + items * elems_per_item / atomic_rate,
+  // t_chunk = the slower of the item's MMA chain and its operand bytes at the per-SM share of L2 bandwidth
+  // (estimates, not measurements: the choice only needs their ratio).
   int splits = 1;
   {
-    const double clk = 1.8e9;
-    const double bytes_chunk = (double)p.pb * (MG * p.mrows + p.TG * p.nblk) * 128.0;
-    const double mma_chunk = (double)p.pb * MG * p.TG * 4.0 * (p.nblk > 64 ? p.nblk : 64) / 256.0 * 222.0;
-    const double t_chunk = (bytes_chunk / 40.0 > mma_chunk ? bytes_chunk / 40.0 : mma_chunk) / clk;
-    const double elems = (double)MG * p.mrows * p.nblk * p.TG;
+    const double clk = 1.7e9, atomic_rate = 60e9;
+    const double bytes_chunk = (double)p.pb * (p.MG * p.mrows + p.TG * NBLK) * 128.0;
+    const double mma_chunk = (double)p.pb * p.MG * p.TG * 4.0 * (NBLK > 64 ? NBLK : 64) / 256.0 * 256.0;
+    const double t_chunk = (bytes_chunk / 32.0 > mma_chunk ? bytes_chunk / 32.0 : mma_chunk) / clk;
+    const double elems = (double)p.MG * p.mrows * NBLK * p.TG;
     const int smax = (2 * sms) / groups > 1 ? (2 * sms) / groups : 1;
     double best = 1e30;
     for (int s = smax; s >= 1; --s) {        // descending: near-ties keep the finer split (better balance)
       if (s > p.chunks_total / 8 && s > 1) continue;
       const int items_s = groups * s, waves = (items_s + sms - 1) / sms;
       const double cpi = (double)((p.chunks_total + s - 1) / s);
-      const double t = waves * cpi * t_chunk + (double)items_s * elems / 90e9;
+      const double t = waves * cpi * t_chunk + (double)items_s * elems / atomic_rate;
       if (t < best * 0.98) { best = t; splits = s; }
     }
   }
-  if (env_get("SPC_WG_SPLIT_CEIL")) splits = (2 * sms + groups - 1) / groups;   // previous behaviour (A/B knob)
   splits = env_int("SPC_WG_SPLITS", splits);
   if (splits > p.chunks_total / 8) splits = p.chunks_total / 8;
   if (splits < 1) splits = 1;
   p.splits = splits;
   p.split_major = env_get("SPC_WG_GROUP_MAJOR") ? 0 : 1;            // A/B knob: previous item order
   const int smem = p.stages * stage_bytes + SMEM_AUX;
-  auto kern = pw_wgrad_kernel<MG>;
+  auto kern = pw_wgrad_kernel<NBLK, NA>;
   static bool attr_set = false;
   if (!attr_set) {
     SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
@@ -926,219 +782,23 @@ int launch_wg(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMap& 
   return SPC_OK;
 }
 
-// ---- wgrad on CTA pairs (cta_group::2), 1x1 convolutions ------------------------------------------
-// Default for 1x1 convolutions with >= 400 input channels (see run_wgrad; verified against the single-CTA
-// kernel and against cuDNN fp32 by tests/test_gpu_fullsize_parity.py).  Why: the single-CTA kernel loads MG*128 + nblk operand rows per 64-pixel chunk for
-// MG*128 x nblk accumulators (e.g. 256 + 240 rows); a pair computes M = 256*MP rows x nblk columns with each
-// CTA loading only ITS 128*MP rows of dY and HALF of the nblk rows of x (256 + 120 rows for the same
-// accumulators per CTA), 24-33 % fewer L2->SM bytes per MAC, and the smaller stage leaves room for 4 stages.
-template <int MP>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS, 1)
-pw_wgrad_pair_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_x,
-                     const WgParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int half = p.nblk / 2;                                // x rows (input channels) this CTA loads
-  const int b_bytes = half * 128;
-  const int b_slot = (b_bytes + 1023) & ~1023;
-  const int stage_bytes = p.pb * (MP * A_BLK_BYTES + b_slot);
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + p.stages * stage_bytes);
-  uint64_t* empty = full + MAX_STAGES;
-  uint64_t* tfull = empty + MAX_STAGES;
-  uint64_t* tempty = tfull + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();                    // 0 = leader (issues the MMAs)
-  const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
-
-  if (threadIdx.x == 0) {
-    // full: leader's arrive.expect_tx + the peer's remote arrive; empty / tfull: one multicast commit;
-    // tempty (used in the leader only): the 128 epilogue threads of each CTA
-    for (int i = 0; i < p.stages; ++i) { mbar_init(&full[i], 2); mbar_init(&empty[i], 1); }
-    mbar_init(tfull, 1);
-    mbar_init(tempty, 256);
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc_2sm(tmem_slot, TMEM_COLS);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const int ngroups = p.mgroups * p.n_blocks;                 // mgroups counts groups of MP row-PAIRS here
-  const int num_items = ngroups * p.splits;
-  const int per_split = (p.chunks_total + p.splits - 1) / p.splits;
-  const uint32_t stage_tx = 2u * (uint32_t)p.pb * (uint32_t)(MP * p.mrows * 128 + b_bytes);   // both CTAs' loads land on the leader's barrier
-
-#define WGP_DECODE(it)                                                          \
-  const int sp = (it) / ngroups;                                               \
-  const int g_ = (it) % ngroups;                                               \
-  const int nb = g_ % p.n_blocks;                                              \
-  const int mgp = g_ / p.n_blocks;                                             \
-  const int c_begin = sp * per_split, c_end = min(p.chunks_total, c_begin + per_split);
-
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmap_dy);
-      tma_prefetch_desc(&tmap_x);
-      int s = 0, ph = 0;
-      for (int it = cluster_id; it < num_items; it += num_clusters) {
-        WGP_DECODE(it)
-        for (int ch = c_begin; ch < c_end; ++ch) {
-          const int n = ch / p.chunks_per_image, p0 = (ch % p.chunks_per_image) * (64 * p.pb);
-          mbar_wait(&empty[s], ph ^ 1);
-          uint8_t* st = smem + s * stage_bytes;
-          if (rank == 0) mbar_arrive_expect_tx(&full[s], stage_tx);
-          else mbar_arrive_cluster(&full[s], 0);
-          if (p.pb == 2) {   // wide stage: 5-d boxes [8-ch group][2 px blocks][8 ch][128 B] (see WgParams::pb)
-#pragma unroll
-            for (int i = 0; i < MP; ++i)
-              tma_load_5d_2sm(st + i * (2 * A_BLK_BYTES), &tmap_dy, &full[s], 0, 0, p0 >> 6,
-                              (((mgp * MP + i) * 2 + (int)rank) * p.mrows) >> 3, n);
-            tma_load_5d_2sm(st + MP * (2 * A_BLK_BYTES), &tmap_x, &full[s], 0, 0, p0 >> 6,
-                            (nb * p.nblk + (int)rank * half) >> 3, n);
-            if (++s == p.stages) { s = 0; ph ^= 1; }
-            continue;
-          }
-#pragma unroll
-          for (int i = 0; i < MP; ++i)      // row pair (mgp*MP + i): this CTA's 128-lane half
-            tma_load_3d_2sm(st + i * A_BLK_BYTES, &tmap_dy, &full[s], p0, ((mgp * MP + i) * 2 + (int)rank) * p.mrows, n);
-          tma_load_3d_2sm(st + MP * A_BLK_BYTES, &tmap_x, &full[s], p0, nb * p.nblk + (int)rank * half, n);
-          if (++s == p.stages) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      const uint32_t idesc = umma_idesc_bf16(256, p.nblk, 0, 0);
-      int s = 0, ph = 0, aph = 0;
-      for (int it = cluster_id; it < num_items; it += num_clusters) {
-        WGP_DECODE(it)
-        (void)nb; (void)mgp;
-        mbar_wait(tempty, aph ^ 1);
-        tc_fence_after();
-        for (int ch = c_begin; ch < c_end; ++ch) {
-          mbar_wait(&full[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * stage_bytes);
-          if (p.pb == 2) {
-            const uint32_t sb = sa + MP * (2 * A_BLK_BYTES);
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-#pragma unroll
-              for (int ks = 0; ks < 4; ++ks) {
-                const uint64_t bdesc = umma_desc(sb + j * 1024 + ks * 32, 16, 2048);
-#pragma unroll
-                for (int i = 0; i < MP; ++i) {
-                  const uint64_t adesc = umma_desc(sa + i * (2 * A_BLK_BYTES) + j * 1024 + ks * 32, 16, 2048);
-                  umma_bf16_2sm(tmem_base + i * p.nblk, adesc, bdesc, idesc, (ch > c_begin || ks > 0 || j > 0) ? 1u : 0u);
-                }
-              }
-            }
-            umma_commit_2sm(&empty[s]);
-            if (++s == p.stages) { s = 0; ph ^= 1; }
-            continue;
-          }
-          const uint32_t sb = sa + MP * A_BLK_BYTES;
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t bdesc = umma_desc(sb + ks * 32, 16, 1024);
-#pragma unroll
-            for (int i = 0; i < MP; ++i) {
-              const uint64_t adesc = umma_desc(sa + i * A_BLK_BYTES + ks * 32, 16, 1024);
-              umma_bf16_2sm(tmem_base + i * p.nblk, adesc, bdesc, idesc, (ch > c_begin || ks > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit_2sm(&empty[s]);
-          if (++s == p.stages) { s = 0; ph ^= 1; }
-        }
-        umma_commit_2sm(tfull);
-        aph ^= 1;
-      }
-    }
-  } else {
-    const int quarter = warp & 3;
-    int aph = 0;
-    for (int it = cluster_id; it < num_items; it += num_clusters) {
-      WGP_DECODE(it)
-      mbar_wait(tfull, aph);
-      tc_fence_after();
-      if (c_end > c_begin) {
-#pragma unroll 1
-        for (int i = 0; i < MP; ++i) {
-          const int rib = quarter * 32 + lane;
-          const int k = rib < p.mrows ? ((mgp * MP + i) * 2 + (int)rank) * p.mrows + rib : p.K;
-#pragma unroll 1
-          for (int cc = 0; cc * 32 < p.nblk; ++cc) {
-            uint32_t r[32];
-            tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + i * p.nblk + cc * 32, r);
-            tmem_ld_wait();
-            if (k < p.K) {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const int cl = cc * 32 + j;
-                const int c = nb * p.nblk + cl;
-                if (cl < p.nblk && c < p.C) atomicAdd(&p.dw[(size_t)k * p.C + c], __uint_as_float(r[j]));
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      mbar_arrive_cluster(tempty, 0);       // both CTAs release the accumulators on the leader's barrier
-      aph ^= 1;
-    }
-  }
-#undef WGP_DECODE
-  tc_fence_before();
-  cluster_sync_all();                       // no CTA may exit while its peer can still signal into it
-  if (warp == 1) tmem_dealloc_2sm(tmem_base, TMEM_COLS);
-}
-
-template <int MP>
-int launch_wg_pair(const CUtensorMap& tdy, const CUtensorMap& tx, WgParams p, cudaStream_t st) {
-  const int b_slot = ((p.nblk / 2) * 128 + 1023) & ~1023;
-  const int stage_bytes = p.pb * (MP * A_BLK_BYTES + b_slot);
-  p.stages = (SMEM_LIMIT - SMEM_AUX) / stage_bytes;
-  if (p.stages > 6) p.stages = 6;
-  p.stages = min(p.stages, env_int("SPC_WG_STAGES", p.stages));
-  SPC_REQUIRE(p.stages >= 2, "tcgen05 pair wgrad: smem budget");
-  const int sms = sm_count();
-  const int clusters = sms / 2;
-  const int groups = p.mgroups * p.n_blocks;
-  int splits = 1;
-  {   // same cost model as launch_wg, per CTA pair
-    const double clk = 1.8e9;
-    const double bytes_chunk = (double)p.pb * (MP * p.mrows + p.nblk / 2) * 128.0;          // per CTA
-    const double mma_chunk = (double)p.pb * MP * 4.0 * (p.nblk > 64 ? p.nblk : 64) / 256.0 * 222.0;
-    const double t_chunk = (bytes_chunk / 40.0 > mma_chunk ? bytes_chunk / 40.0 : mma_chunk) / clk;
-    const double elems = 2.0 * MP * p.mrows * p.nblk;
-    const int smax = (2 * clusters) / groups > 1 ? (2 * clusters) / groups : 1;
-    double best = 1e30;
-    for (int s = smax; s >= 1; --s) {
-      if (s > p.chunks_total / 8 && s > 1) continue;
-      const int items_s = groups * s, waves = (items_s + clusters - 1) / clusters;
-      const double cpi = (double)((p.chunks_total + s - 1) / s);
-      const double t = waves * cpi * t_chunk + (double)items_s * elems / 90e9;
-      if (t < best * 0.98) { best = t; splits = s; }
-    }
-  }
-  splits = env_int("SPC_WG_SPLITS", splits);
-  if (splits > p.chunks_total / 8) splits = p.chunks_total / 8;
-  if (splits < 1) splits = 1;
-  p.splits = splits;
-  const int smem = p.stages * stage_bytes + SMEM_AUX;
-  auto kern = pw_wgrad_pair_kernel<MP>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
-    attr_set = true;
-  }
-  const int items = groups * p.splits;
-  const int grid = 2 * (items < clusters ? items : clusters);
-  kern<<<grid, TC_THREADS, smem, st>>>(tdy, tx, p);
-  count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  return SPC_OK;
+// accumulators per item: MG dY blocks x TG taps, a power of two <= WG_ACC / NBLK.  TG: all taps when they fit, else the
+// most that fit the accumulator registers and leave room for >= 2 pipeline stages
+template <int NBLK>
+int launch_wg_na(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMap& tx4, const WgParams& p, cudaStream_t st) {
+  constexpr int NACC = WG_ACC / NBLK;
+  const int b_slot = (NBLK * 128 + 1023) & ~1023;
+  int na = p.MG;
+  while (na * 2 <= NACC && na / p.MG < p.taps &&
+         p.MG * A_BLK_BYTES + (na * 2 / p.MG) * b_slot <= (SMEM_LIMIT - SMEM_AUX) / 2)
+    na *= 2;
+  if (na == 1) return launch_wg<NBLK, 1>(tdy, tx, tx4, p, st);
+  if (na == 2) return launch_wg<NBLK, 2>(tdy, tx, tx4, p, st);
+  if constexpr (NACC >= 4) { if (na == 4) return launch_wg<NBLK, 4>(tdy, tx, tx4, p, st); }
+  if constexpr (NACC >= 8) { if (na == 8) return launch_wg<NBLK, 8>(tdy, tx, tx4, p, st); }
+  if constexpr (NACC >= 16) { if (na == 16) return launch_wg<NBLK, 16>(tdy, tx, tx4, p, st); }
+  set_error("wgmma wgrad: no kernel for %d accumulators of %d channels", na, NBLK);
+  return SPC_EUNSUPPORTED;
 }
 
 // x: activations [N][C][Hin][Wo] (taps == 1: Hin == Ho) or their S column-shifted (and, for
@@ -1149,43 +809,41 @@ int run_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, int K,
   WgParams p{};
   p.dw = dw; p.K = K; p.C = C; p.P = P; p.N = N;
   p.taps = R * S; p.S = S; p.ph = ph; p.W = Wo; p.shiftN = copies ? N : 0; p.rowmul = stride;
-  const int nblk_max = min(256, round_up(env_int("SPC_WG_NBLK", 256), 16));   // accumulator width (input channels)
-  p.n_blocks = (C + nblk_max - 1) / nblk_max;
-  p.nblk = round_up((C + p.n_blocks - 1) / p.n_blocks, 16);
+  // accumulator width (input channels): C split evenly over blocks of <= 128, rounded up to an instantiated width
+  p.n_blocks = (C + 127) / 128;
+  {
+    const int w = round_up((C + p.n_blocks - 1) / p.n_blocks, 16);
+    p.nblk = w <= 16 ? 16 : (w <= 32 ? 32 : (w <= 64 ? 64 : 128));
+  }
   int MBtot = (K + 127) / 128;
   p.mrows = env_get("SPC_WG_ROWS128") ? 128 : round_up((K + MBtot - 1) / MBtot, 8);   // e.g. K = 416 -> 4 blocks of 104
   MBtot = (K + p.mrows - 1) / p.mrows;
-  int MG = p.taps > 1 ? 1 : 512 / p.nblk;
+  int MG = p.taps > 1 ? 1 : WG_ACC / p.nblk;
   if (MG > MBtot) MG = MBtot;
   MG = min(MG, env_int("SPC_WG_MG", MG));
   MG = MG >= 4 ? 4 : (MG >= 2 ? 2 : 1);
-  p.mgroups = (MBtot + MG - 1) / MG;
   p.chunks_per_image = (P + 63) / 64;
   p.chunks_total = p.chunks_per_image * N;
   p.pb = 1;
-  // CTA pairs (cta_group::2): measured on B200 (tools/wgrad_probe.py --pair, profiles/r2_wgrad_pair.txt): x1.11..1.32
-  // for >= 416 input channels (624->416 @2048^2: 4.95 -> 3.74 ms), break-even at 416->104 / 208->52, slower for
-  // the HBM-bound narrow layers (104->208: x0.75, 52->208: x0.67).  SPC_WG_2CTA=1 / SPC_WG_1CTA=1 force either.
-  const bool pair = p.taps == 1 && (env_get("SPC_WG_2CTA") ? true : (env_get("SPC_WG_1CTA") ? false : C >= 400)) &&
-                    MBtot >= 2 && p.nblk % 16 == 0;
   // wide stages (two 64-pixel blocks per operand row and stage, 5-d boxes): for 1x1 layers whose channel planes span
   // several 2 MB pages, same reason as PwParams::x5.  SPC_WG_WIDE=0/1 overrides, SPC_WG_BOX5 (bit 0 dy, bit 1 x).
   {
     const char* we = env_get("SPC_WG_WIDE");
-    const bool wide = p.taps == 1 && !pair && P % 128 == 0 && (we ? atoi(we) != 0 : (size_t)P * 2 >= ((size_t)2 << 20));
+    const bool wide = p.taps == 1 && P % 128 == 0 && (we ? atoi(we) != 0 : (size_t)P * 2 >= ((size_t)2 << 20));
     if (wide) {
       const int b_slot = (p.nblk * 128 + 1023) & ~1023;
       while (MG > 1 && 2 * 2 * (MG * A_BLK_BYTES + b_slot) > SMEM_LIMIT - SMEM_AUX) MG >>= 1;
-      p.mgroups = (MBtot + MG - 1) / MG;
       p.pb = 2;
       p.chunks_per_image = P / 128;
       p.chunks_total = p.chunks_per_image * N;
       const char* be = env_get("SPC_WG_BOX5");
       const int b5 = be ? atoi(be) : 3;
       p.dy5 = ((b5 & 1) && K % 8 == 0 && p.mrows % 8 == 0) ? 1 : 0;
-      p.x5 = ((b5 & 2) && C % 8 == 0 && p.nblk % 8 == 0) ? 1 : 0;
+      p.x5 = ((b5 & 2) && C % 8 == 0) ? 1 : 0;
     }
   }
+  p.MG = MG;
+  p.mgroups = (MBtot + MG - 1) / MG;
   CUtensorMap tdy, tx, tx4;
   int rc = p.dy5 ? make_act_tmap5(&tdy, dy, P, K, N, p.mrows / 8, 2) : make_act_tmap(&tdy, dy, P, K, N, p.mrows);
   if (rc) return rc;
@@ -1201,38 +859,10 @@ int run_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, int K,
     if (rc) return rc;
     tx4 = tx;
   }
-  if (pair) {
-    // CTA pairs (see pw_wgrad_pair_kernel): row pairs of 2*mrows, MP pairs per item.  Wide stages (5-d boxes, see
-    // WgParams::pb) measured x1.34..1.64 on every pair layer of the list (profiles/r2f_wgrad_pairwide.txt:
-    // 1664->416 @1024^2 2.05 -> 1.53 ms = 948 TFLOP/s, 624->416 @2048^2 4.05 -> 2.54 ms); SPC_WG_PAIR_WIDE=0/1 overrides.
-    const int npairs = (MBtot + 1) / 2;
-    int MP = 512 / p.nblk;
-    if (MP > npairs) MP = npairs;
-    MP = MP >= 2 ? 2 : 1;
-    CUtensorMap txh;      // x boxes of nblk/2 channels: each CTA of a pair loads its half of the block
-    const char* we = env_get("SPC_WG_PAIR_WIDE");
-    const bool wide = P % 128 == 0 && K % 8 == 0 && C % 8 == 0 && p.mrows % 8 == 0 && p.nblk % 16 == 0 &&
-                      (we ? atoi(we) != 0 : (size_t)P * 2 >= ((size_t)2 << 20));
-    if (wide) {
-      const int b_slot = ((p.nblk / 2) * 128 + 1023) & ~1023;
-      if (MP == 2 && env_get("SPC_WG_PAIR_MP1")) MP = 1;
-      while (MP > 1 && 2 * 2 * (MP * A_BLK_BYTES + b_slot) > SMEM_LIMIT - SMEM_AUX) MP >>= 1;
-      p.pb = 2;
-      p.chunks_per_image = P / 128;
-      p.chunks_total = p.chunks_per_image * N;
-      rc = make_act_tmap5(&tdy, dy, P, K, N, p.mrows / 8, 2);
-      if (rc) return rc;
-      rc = make_act_tmap5(&txh, x, P, C, N, p.nblk / 16, 2);
-    } else {
-      rc = make_act_tmap(&txh, x, P, C, N, p.nblk / 2);
-    }
-    if (rc) return rc;
-    p.mgroups = (npairs + MP - 1) / MP;
-    return MP == 2 ? launch_wg_pair<2>(tdy, txh, p, st) : launch_wg_pair<1>(tdy, txh, p, st);
-  }
-  if (MG == 1) return launch_wg<1>(tdy, tx, tx4, p, st);
-  if (MG == 2) return launch_wg<2>(tdy, tx, tx4, p, st);
-  return launch_wg<4>(tdy, tx, tx4, p, st);
+  if (p.nblk == 16) return launch_wg_na<16>(tdy, tx, tx4, p, st);
+  if (p.nblk == 32) return launch_wg_na<32>(tdy, tx, tx4, p, st);
+  if (p.nblk == 64) return launch_wg_na<64>(tdy, tx, tx4, p, st);
+  return launch_wg_na<128>(tdy, tx, tx4, p, st);
 }
 
 // ---- 3x3 stride-2 dgrad: the four output-parity classes of dX as channel groups of ONE 2x2-tap
@@ -1326,7 +956,7 @@ __global__ void upsample2_zero_kernel(const __nv_bfloat16* __restrict__ g, __nv_
 int launch_resample(bool up, const void* src, void* dst, size_t planes, int H, int W, cudaStream_t st) {
   const size_t total = planes * (H / 2) * (W / 16);
   size_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   if (up)
     upsample2_zero_kernel<<<(int)blocks, 256, 0, st>>>((const __nv_bfloat16*)src, (__nv_bfloat16*)dst, planes, H, W);
   else
@@ -1336,7 +966,7 @@ int launch_resample(bool up, const void* src, void* dst, size_t planes, int H, i
   return SPC_OK;
 }
 
-// TMA tile loads need 16-byte aligned inner coordinates (measured: tools/tma_probe.cu), so the
+// TMA tile loads need 16-byte aligned inner coordinates, so the
 // horizontal taps of an R x S filter cannot be fetched as shifted boxes.  For S > 1 one pre-pass
 // writes the S column-shifted, zero-filled copies  xs[s][plane][h][w] = x[plane][h][w + s - pw];
 // every tap (r, s) is then an ALIGNED box of copy s at row offset r - ph.
@@ -1434,7 +1064,7 @@ int launch_shift_copies(const void* x, void* xs, size_t planes, int H, int W, in
       ((S == 7 && pw == 3) || (S == 3 && pw == 1) || (S == 5 && pw == 2) || (S == 2 && pw == 0))) {
     const size_t tot = planes * H * (W / 8);
     size_t blocks = (tot + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     const __nv_bfloat16* xi = (const __nv_bfloat16*)x;
     __nv_bfloat16* xo = (__nv_bfloat16*)xs;
     if (S == 7) shift_copies_vec_kernel<7, 3><<<(int)blocks, 256, 0, st>>>(xi, xo, planes, H, W);
@@ -1448,7 +1078,7 @@ int launch_shift_copies(const void* x, void* xs, size_t planes, int H, int W, in
   if (aligned && cs == 2 && S == 3 && pw == 1 && W % 16 == 0) {
     const size_t tot = planes * H * (W / 16);
     size_t blocks = (tot + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     shift_copies_s2k3_kernel<<<(int)blocks, 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)xs, planes, H, W);
     count_launch();
     SPC_CHECK_CUDA(cudaGetLastError());
@@ -1456,7 +1086,7 @@ int launch_shift_copies(const void* x, void* xs, size_t planes, int H, int W, in
   }
   const size_t total = planes * H * (W / cs / 8) * S;
   size_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   shift_copies_kernel<<<(int)blocks, 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)xs, planes, H, W, S, pw, cs);
   count_launch();
   SPC_CHECK_CUDA(cudaGetLastError());
@@ -1538,7 +1168,7 @@ size_t tc_workspace_bytes(const spc_conv_desc* d, int op) {
 
 int tc_conv_fwd(const spc_conv_desc* d, const void* x, const void* w, const void* bias, void* y, void* ws,
                 size_t ws_bytes, cudaStream_t st) {
-  SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 0), "tcgen05 conv: workspace too small");
+  SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 0), "wgmma conv: workspace too small");
   if (d->R * d->S > 1) {
     TcConv c{};
     c.w = reinterpret_cast<const __nv_bfloat16*>(w);
@@ -1564,7 +1194,7 @@ int tc_conv_fwd(const spc_conv_desc* d, const void* x, const void* w, const void
 int tc_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* dx, void* ws, size_t ws_bytes,
                   cudaStream_t st) {
   // dX[C x P] = W^T[C x K] * dY[K x P]
-  SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 1), "tcgen05 conv: workspace too small");
+  SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 1), "wgmma conv: workspace too small");
   if (d->R * d->S > 1 && is_s2(d)) {   // 3x3 stride 2: four parity classes as channel groups, then interleave
     const int Ho = d->H / 2, Wo = d->W / 2;
     const int Mq = 4 * d->C, Mpad = round_up(Mq, 128), Kpad = round_up(d->K, BK);
@@ -1589,7 +1219,7 @@ int tc_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* d
     if (rc) return rc;
     const size_t total = (size_t)d->N * d->C * 2 * Ho * (Wo / 8);
     size_t blocks = (total + 255) / 256;
-    if (blocks > 148 * 32) blocks = 148 * 32;
+    if (blocks > 132 * 32) blocks = 132 * 32;
     interleave_s2_kernel<<<(int)blocks, 256, 0, st>>>(tmp, reinterpret_cast<__nv_bfloat16*>(dx), d->N, d->C, Ho, Wo);
     count_launch();
     SPC_CHECK_CUDA(cudaGetLastError());
@@ -1629,7 +1259,7 @@ int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* 
       return run_wgrad_tap(xb, dyb, dw, d->K, d->C, d->N, d->H, d->W, d->R, d->S, st);
     const bool copies = d->S > 1 || cs > 1;
     if (copies) {
-      SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 2), "tcgen05 wgrad: workspace too small");
+      SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 2), "wgmma wgrad: workspace too small");
       void* xs = reinterpret_cast<void*>(align1k(reinterpret_cast<uintptr_t>(ws)));
       int rc = launch_shift_copies(x, xs, (size_t)d->N * d->C, d->H, d->W, d->S, d->pad_w, cs, st);
       if (rc) return rc;
@@ -1638,7 +1268,7 @@ int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* 
     return run_wgrad(xb, dyb, dw, d->K, d->C, d->N, d->H / cs, d->W / cs, d->H, d->R, d->S, d->pad_h, cs, copies, st);
   }
   if (is_s2(d)) {
-    SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 2), "tcgen05 wgrad: workspace too small");
+    SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 2), "wgmma wgrad: workspace too small");
     void* xs = reinterpret_cast<void*>(align1k(reinterpret_cast<uintptr_t>(ws)));
     int rc = launch_resample(false, x, xs, (size_t)d->N * d->C, d->H, d->W, st);
     if (rc) return rc;
@@ -1649,7 +1279,7 @@ int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* 
 }
 
 // Y[M][P] = W[M][Cin] * X[Cin][P] (bf16; w row-major with leading dimension ld) and dW[K][C] += dY[K][P] * X[C][P]^T on
-// the pointwise tcgen05 kernels -- used by the halo fix-up (api.cu), where "channels" are (c, r, s) triples of the
+// the pointwise wgmma kernels -- used by the halo fix-up (api.cu), where "channels" are (c, r, s) triples of the
 // filter and "pixels" are the boundary outputs
 size_t tc_pw_workspace_bytes(int M, int Cin) { return (size_t)round_up(M, 128) * round_up(Cin, BK) * 2 + 4096; }
 int tc_pw_fwd(const void* w, int ld, int M, int Cin, const void* x, const void* bias, void* y, int P, void* ws, size_t ws_bytes,
@@ -1671,5 +1301,5 @@ int tc_sm_count() { return sm_count(); }
 
 }  // namespace spc
 
-// tuning probes (tools/wgrad_probe.py) change SPC_* knobs inside one process: forget the cached values
+// tuning probes change SPC_* knobs inside one process: forget the cached values
 extern "C" void spc_reload_env(void) { spc::g_env_n = 0; }

@@ -346,7 +346,7 @@ __global__ void boundary_scatter_kernel(const __nv_bfloat16* __restrict__ O, con
 
 inline int grid_for(size_t total) {
   size_t b = (total + 255) / 256;
-  if (b > 148 * 16) b = 148 * 16;
+  if (b > 132 * 16) b = 132 * 16;
   if (b < 1) b = 1;
   return (int)b;
 }
@@ -433,8 +433,8 @@ int spc_device_info(int device, int* sm_count, int* cc) {
   SPC_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
   if (sm_count) *sm_count = prop.multiProcessorCount;
   if (cc) *cc = prop.major * 10 + prop.minor;
-  SPC_REQUIRE(prop.major == 10, "libspconv is built for sm_100a only; device %d is sm_%d%d", device, prop.major,
-              prop.minor);
+  SPC_REQUIRE(prop.major == 9 && prop.minor == 0, "libspconv is built for sm_90a only; device %d is sm_%d%d", device,
+              prop.major, prop.minor);
   return SPC_OK;
 }
 

@@ -1,4 +1,4 @@
-// pool.cu -- spatially-partitioned Max/Avg pooling forward and backward for sm_100a.
+// pool.cu -- spatially-partitioned Max/Avg pooling forward and backward for sm_90a.
 //
 // Replaces Pool.forward (reference spatial.py:1503-1509): halo_exchange_layer (pad + 8-way
 // exchange + 8 unpack copies) followed by nn.{Max,Avg}Pool2d(padding=0).  Here the window is
@@ -531,7 +531,7 @@ int launch_pool3_tma(const PoolParams& p, cudaStream_t st) {
     SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM_BYTES));
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
     attr_set = true;
   }
   const int grid = nt < (size_t)(2 * sms) ? (int)nt : 2 * sms;
@@ -543,7 +543,7 @@ int launch_pool3_tma(const PoolParams& p, cudaStream_t st) {
   if (halos) {
     const int ring = 2 * p.in.W + 2 * p.in.H;
     const size_t total = planes * ring;
-    const int blocks = (int)((total + 255) / 256 > 148 * 8 ? 148 * 8 : (total + 255) / 256);
+    const int blocks = (int)((total + 255) / 256 > 132 * 8 ? 132 * 8 : (total + 255) / 256);
     pool3_s1_ring_kernel<T><<<blocks, 256, 0, st>>>(p);
     count_launch();
     SPC_CHECK_CUDA(cudaGetLastError());
@@ -688,7 +688,7 @@ int run_fwd(const PoolParams& p, cudaStream_t st) {
   const bool vec_ok = aligned && p.Wo % VEC == 0 && p.in.W % (VEC * p.stride) == 0 &&
                       p.in.W == p.Wo * p.stride;
   const size_t vtotal = total / VEC;
-  const int blocks = (int)((vtotal + 255) / 256 > 148 * 32 ? 148 * 32 : (vtotal + 255) / 256);
+  const int blocks = (int)((vtotal + 255) / 256 > 132 * 32 ? 132 * 32 : (vtotal + 255) / 256);
   if (vec_ok && p.k == 3 && p.stride == 1 && pool3_tma_ok<T>(p)) {
     return launch_pool3_tma<T>(p, st);
   } else if (vec_ok && p.k == 3 && p.stride == 1 && p.in.W % (VEC * 32) != 0) {
@@ -698,14 +698,14 @@ int run_fwd(const PoolParams& p, cudaStream_t st) {
   } else if (vec_ok && p.k == 3 && p.stride == 1) {
     constexpr int RB = 16;
     const size_t items = (size_t)p.in.N * p.in.C * ((p.in.H + RB - 1) / RB) * (p.in.W / VEC);
-    const int b3 = (int)((items + 255) / 256 > 148 * 16 ? 148 * 16 : (items + 255) / 256);
+    const int b3 = (int)((items + 255) / 256 > 132 * 16 ? 132 * 16 : (items + 255) / 256);
     pool3_s1_rolling_kernel<T, VEC, RB><<<b3, 256, 0, st>>>(p);
   } else if (vec_ok && p.k == 3 && p.stride == 2) {
     pool3_fwd_kernel<T, VEC, 2><<<blocks, 256, 0, st>>>(p);
   } else if (vec_ok && p.k == 2 && p.stride == 2) {
     pool_fwd_vec_kernel<T, VEC, 2, 2><<<blocks, 256, 0, st>>>(p);
   } else {
-    const int b2 = (int)((total + 255) / 256 > 148 * 32 ? 148 * 32 : (total + 255) / 256);
+    const int b2 = (int)((total + 255) / 256 > 132 * 32 ? 132 * 32 : (total + 255) / 256);
     pool_fwd_kernel<T><<<b2, 256, 0, st>>>(p);
   }
   spc::count_launch();
@@ -717,7 +717,7 @@ template <typename T>
 int run_bwd(const PoolParams& p, cudaStream_t st) {
   const size_t total = (size_t)p.in.N * p.in.C * p.in.H * p.in.W;
   if (total == 0) return SPC_OK;
-  const int blocks = (int)((total + 255) / 256 > 148 * 32 ? 148 * 32 : (total + 255) / 256);
+  const int blocks = (int)((total + 255) / 256 > 132 * 32 ? 132 * 32 : (total + 255) / 256);
   const bool aligned = ((uintptr_t)p.in.x % 16 == 0) && ((uintptr_t)p.out % 16 == 0) && ((uintptr_t)p.dy % 16 == 0);
   const bool even = aligned && p.in.W % 16 == 0 && p.in.H % 2 == 0 && p.in.W == 2 * p.Wo && p.in.H == 2 * p.Ho;
   if (p.mode == SPC_POOL_AVG && p.k == 3 && p.stride == 1 && aligned && p.in.W % (16 / sizeof(T)) == 0) {
@@ -729,19 +729,19 @@ int run_bwd(const PoolParams& p, cudaStream_t st) {
     const size_t vt = total / VEC;
     constexpr int RB = 16;
     const size_t items = (size_t)q.in.N * q.in.C * ((q.in.H + RB - 1) / RB) * (q.in.W / VEC);
-    const int b2 = (int)((items + 255) / 256 > 148 * 16 ? 148 * 16 : (items + 255) / 256);
-    const int b1 = (int)((vt + 255) / 256 > 148 * 32 ? 148 * 32 : (vt + 255) / 256);
+    const int b2 = (int)((items + 255) / 256 > 132 * 16 ? 132 * 16 : (items + 255) / 256);
+    const int b1 = (int)((vt + 255) / 256 > 132 * 32 ? 132 * 32 : (vt + 255) / 256);
     if (pool3_tma_ok<T>(q)) return launch_pool3_tma<T>(q, st);
     if (getenv("SPC_POOL_SIMPLE") != nullptr) pool3_s1_simple_kernel<T, VEC><<<b1, 256, 0, st>>>(q);
     else if (q.in.W % (VEC * 32) == 0) pool3_s1_rolling_kernel<T, VEC, RB><<<b2, 256, 0, st>>>(q);
     else pool3_fwd_kernel<T, VEC, 1><<<b1, 256, 0, st>>>(q);
   } else if (even && p.mode == SPC_POOL_AVG && p.k == 3 && p.stride == 2) {
     const size_t vt = total / 32;
-    const int b2 = (int)((vt + 255) / 256 > 148 * 32 ? 148 * 32 : (vt + 255) / 256);
+    const int b2 = (int)((vt + 255) / 256 > 132 * 32 ? 132 * 32 : (vt + 255) / 256);
     pool_bwd_s2_vec_kernel<T, SPC_POOL_AVG><<<b2, 256, 0, st>>>(p);
   } else if (even && p.mode == SPC_POOL_MAX && p.k == 2 && p.stride == 2) {
     const size_t vt = total / 32;
-    const int b2 = (int)((vt + 255) / 256 > 148 * 32 ? 148 * 32 : (vt + 255) / 256);
+    const int b2 = (int)((vt + 255) / 256 > 132 * 32 ? 132 * 32 : (vt + 255) / 256);
     pool_bwd_s2_vec_kernel<T, SPC_POOL_MAX><<<b2, 256, 0, st>>>(p);
   } else {
     pool_bwd_kernel<T><<<blocks, 256, 0, st>>>(p);

@@ -1,20 +1,22 @@
-// wgrad_tap.cu -- weight gradient of the multi-tap stride-1 convolutions (1x7 / 7x1 / 3x3) on tcgen05, with the
+// wgrad_tap.cu -- weight gradient of the multi-tap stride-1 convolutions (1x7 / 3x3 / 5x5) on wgmma, with the
 // horizontally shifted operand formed in shared memory -- the wgrad counterpart of conv_tap.cu; replaces round 1's
 // pw_wgrad_kernel over S column-shifted HBM copies of the input for these shapes.
 //
 //     dW[k][c][r][s] = sum_{n,h,w} dY[n][k][h][w] * X[n][c][h + r - ph][w + s - pw]          (pixels = reduction dim)
 //
 // Both operands are K-major straight from NCHW (64 contiguous pixels of a row = one 128-byte swizzle row per channel).
-// P operand (M side, TMEM lanes) = the tensor with MORE channels, unshifted, loaded by TMA as it is;
-// Q operand (N side, TMEM columns) = the other tensor: every row is loaded ONCE with 8 pixels of slack (aligned box),
-// and the shifter warps write its S column-shifted tiles [Qch][64 px] next to each other in shared memory, so one MMA
-// with N = S * Qch columns covers a whole filter row.  mode A: P = dY, Q = X;  mode B: P = X, Q = dY, which is mode A
+// P operand (M side, accumulator rows) = the tensor with MORE channels, unshifted, loaded by TMA as it is;
+// Q operand (N side, accumulator columns) = the other tensor: every row is loaded ONCE with 8 pixels of slack (aligned
+// box), and the shifter warps write its S column-shifted tiles [Qch][64 px] next to each other in shared memory; one
+// wgmma (N = QC = Qch rounded up to 16) per tap.  mode A: P = dY, Q = X;  mode B: P = X, Q = dY, which is mode A
 // with both tap indices mirrored (dW[k][c][R-1-r][S-1-s]).
 // Line buffer: a CTA walks down a 64-pixel-wide column strip; step j = P row ha + j meets Q rows j .. j + R' - 1 of a
-// ring of shifted row tile-sets, so every Q row is loaded and shifted once and used by R' steps.  Accumulators of all
-// taps of a pass live in TMEM (<= 512 columns; more taps -> more passes over the strip); fp32 atomics at the end.
+// ring of shifted row tile-sets, so every Q row is loaded and shifted once and used by R' steps.  Accumulators of the
+// NT = 128 / QC taps of a pass live in the registers of two consumer warpgroups (64 fp32 per thread; more taps -> more
+// passes over the strip); fp32 atomics at the end.  Every k-step issues all NT wgmma (the last pass may have fewer
+// taps: its spare accumulators repeat the last tap and are not flushed), so none sits under a data-dependent branch.
 //
-// Warp roles (448 threads): 0 = TMA producer, 1 = MMA issuer (+TMEM alloc), 2..5 = flush, 6..13 = shifter.
+// Warp roles (640 threads): 0 = TMA producer, 4..11 = two consumer warpgroups (wgmma + flush), 12..19 = shifter.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -30,7 +32,7 @@ int tc_sm_count();
 
 namespace {
 
-constexpr int WT_THREADS = 448;
+constexpr int WT_THREADS = 640;
 constexpr int SHIFT_THREADS = 256;
 constexpr int RAW_ROW = 160;       // raw Q row: [Qch][80 px], dense rows of 160 bytes
 constexpr int MAXP = 8;            // P row stages (ring depths are chosen by the launcher: bytes in flight)
@@ -100,10 +102,11 @@ struct ShiftCols {
   }
 };
 
-template <int S>
+template <int S, int QC>
 __global__ void __launch_bounds__(WT_THREADS, 1)
 wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constant__ CUtensorMap tmap_q, const WtParams p) {
   constexpr bool SHIFT = S > 1;
+  constexpr int NT = 128 / QC;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int qblk_bytes = p.ns * p.qt_bytes;                 // the shifted tiles of one 64-pixel block of a Q row
@@ -120,24 +123,16 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
   uint64_t* qt_empty = qt_full + MAXQ;
   uint64_t* raw_full = qt_empty + MAXQ;
   uint64_t* raw_empty = raw_full + MAXRAW;
-  uint64_t* tfull = raw_empty + MAXRAW;
-  uint64_t* tempty = tfull + 1;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < MAXP; ++i) { mbar_init(&p_full[i], 1); mbar_init(&p_empty[i], 1); }
-    for (int i = 0; i < MAXQ; ++i) { mbar_init(&qt_full[i], SHIFT ? SHIFT_THREADS : 1); mbar_init(&qt_empty[i], 1); }
+    // p_empty / qt_empty: one arrive per consumer warpgroup
+    for (int i = 0; i < MAXP; ++i) { mbar_init(&p_full[i], 1); mbar_init(&p_empty[i], 2); }
+    for (int i = 0; i < MAXQ; ++i) { mbar_init(&qt_full[i], SHIFT ? SHIFT_THREADS : 1); mbar_init(&qt_empty[i], 2); }
     for (int i = 0; i < MAXRAW; ++i) { mbar_init(&raw_full[i], 1); mbar_init(&raw_empty[i], SHIFT_THREADS); }
-    mbar_init(tfull, 1);
-    mbar_init(tempty, 128);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // item -> (image n, column strip, row range [ha, hb))
 #define WT_ITEM(it)                                                               \
@@ -187,61 +182,10 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      Ring qr, pr;          // qr.i = ring index of Q row 0 of the current item
-      int tph = 0;
-      const int ngrp = (p.ns * p.Qc16 + 255) / 256;                 // MMAs per filter row (N <= 256 each)
-      const int ns_g = (p.ns + ngrp - 1) / ngrp;                    // filter columns per MMA
-      for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
-        WT_ITEM(it)
-        (void)w0; (void)n_; (void)q_first;
-        if (rows <= 0) continue;
-        mbar_wait(tempty, tph ^ 1);
-        tc_fence_after();
-        for (int j = 0; j < rows; ++j) {
-          // Q rows j .. j + nr - 1 must have landed: all of them at the first step, then one new row per step
-          for (int i = (j == 0 ? 0 : p.nr - 1); i < p.nr; ++i) {
-            const int g = qr.i + j + i;
-            mbar_wait(&qt_full[g % p.rq], (g / p.rq) & 1);
-          }
-          const int ps = pr.slot(p.psn);
-          mbar_wait(&p_full[ps], pr.phase(p.psn));
-          tc_fence_after();
-          for (int b = 0; b < p.nbw; ++b) {
-            const uint32_t sa = smem_u32(p_base + ps * prow_bytes + b * p.p_blk);
-            for (int r = 0; r < p.nr; ++r) {
-              const int g = qr.i + j + r;
-              const uint32_t sq = smem_u32(qt_base + (g % p.rq) * qrow_bytes + b * qblk_bytes);
-              for (int sg = 0; sg * ns_g < p.ns; ++sg) {
-                const int nsg = min(ns_g, p.ns - sg * ns_g);
-                const uint32_t idesc = umma_idesc_bf16(128, nsg * p.Qc16, 0, 0);
-                const uint32_t dcol = tmem_base + (uint32_t)((r * p.ns + sg * ns_g) * p.Qc16);
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) {   // 64 pixels = 4 k-steps of 16; +32 bytes inside the 128-byte swizzle row
-                  const uint64_t adesc = umma_desc(sa + ks * 32, 16, 1024);
-                  const uint64_t bdesc = umma_desc(sq + sg * ns_g * p.qt_bytes + ks * 32, 16, 1024);
-                  umma_bf16(dcol, adesc, bdesc, idesc, (j | b | ks) ? 1u : 0u);
-                }
-              }
-            }
-          }
-          umma_commit(&p_empty[ps]);
-          ++pr.i;
-          { const int g = qr.i + j; umma_commit(&qt_empty[g % p.rq]); }   // Q row j: step j was its last use (r = 0)
-        }
-        // rows j = rows .. rows + nr - 2 of the ring were loaded for the last steps and are dead now: release them
-        for (int i = rows; i < q_rows; ++i) { const int g = qr.i + i; umma_commit(&qt_empty[g % p.rq]); }
-        qr.i += q_rows;
-        umma_commit(tfull);
-        tph ^= 1;
-      }
-    }
-  } else if (warp >= 6) {
+  } else if (warp >= 12) {
     // ================= shifter: raw Q row -> S' shifted K-major tiles =================
     if (SHIFT) {
-      const int tid = threadIdx.x - 6 * 32;
+      const int tid = threadIdx.x - 12 * 32;
       const int q = tid & 7, c0 = tid >> 3;
       Ring qr, rr;
       for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
@@ -280,57 +224,98 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
         }
       }
     }
-  } else if (warp >= 2 && warp <= 5) {
-    // ================= flush: TMEM -> fp32 atomics on dW =================
-    const int quarter = warp & 3;
-    const int pl = quarter * 32 + lane;        // P channel = TMEM lane
-    int tph = 0;
+  } else if (threadIdx.x >= 128) {
+    // ================= consumers: wgmma over (row step, 64-pixel block, tap), then fp32 atomics on dW =================
+    const int wg = (threadIdx.x >> 7) - 1;
+    const int w4 = (threadIdx.x >> 5) & 3;
+    const bool wg_lead = (threadIdx.x & 127) == 0;
+    const int ntaps = p.nr * p.ns;
+    float acc[NT][QC / 2];
+    Ring qr, pr;          // qr.i = ring index of Q row 0 of the current item
     for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
       WT_ITEM(it)
-      (void)w0; (void)n_; (void)q_first; (void)q_rows;
+      (void)w0; (void)n_; (void)q_first;
       if (rows <= 0) continue;
-      mbar_wait(tfull, tph);
-      tc_fence_after();
-      const int ncols = p.nr * p.ns * p.Qc16;
-#pragma unroll 1
-      for (int c32 = 0; c32 < ncols; c32 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(quarter * 32) << 16) + c32, v);
-        tmem_ld_wait();
-        if (pl < p.Pch) {
+      int rel_p = -1, rel_q = -1;             // slots read by the last committed wgmma group
+      for (int j = 0; j < rows; ++j) {
+        // Q rows j .. j + nr - 1 must have landed: all of them at the first step, then one new row per step
+        for (int i = (j == 0 ? 0 : p.nr - 1); i < p.nr; ++i) {
+          const int g = qr.i + j + i;
+          mbar_wait(&qt_full[g % p.rq], (g / p.rq) & 1);
+        }
+        const int ps = pr.slot(p.psn);
+        mbar_wait(&p_full[ps], pr.phase(p.psn));
+        wgmma_fence();
+        for (int b = 0; b < p.nbw; ++b) {
+          const uint32_t sa = smem_u32(p_base + ps * prow_bytes + b * p.p_blk) + wg * 8192;
 #pragma unroll
-          for (int e = 0; e < 32; ++e) {
-            const int col = c32 + e;
-            if (col < ncols) {
-              const int tap = col / p.Qc16, qc = col - tap * p.Qc16;
-              if (qc < p.Qch) {
-                int r = p.r0 + tap / p.ns, s = p.s0 + tap % p.ns;
-                int k, c;
-                if (p.modeB) { k = qc; c = pl; r = p.R - 1 - r; s = p.S - 1 - s; } else { k = pl; c = qc; }
-                atomicAdd(&p.dw[(((size_t)k * p.C + c) * p.R + r) * p.S + s], __uint_as_float(v[e]));
+          for (int a = 0; a < NT; ++a) {
+            const int ta = min(a, ntaps - 1);
+            const int r = ta / p.ns, si = ta - r * p.ns;
+            const int g = qr.i + j + r;
+            const uint32_t sq = smem_u32(qt_base + (g % p.rq) * qrow_bytes + b * qblk_bytes + si * p.qt_bytes);
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks)   // 64 pixels = 4 k-steps of 16; +32 bytes inside the 128-byte swizzle row
+              Wgmma<QC, 0>::mma(acc[a], gmma_desc(sa + ks * 32, 16, 1024), gmma_desc(sq + ks * 32, 16, 1024),
+                                (j | b | ks) ? 1u : 0u);
+          }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (wg_lead) {
+          if (rel_p >= 0) mbar_arrive(&p_empty[rel_p]);
+          if (rel_q >= 0) mbar_arrive(&qt_empty[rel_q]);
+        }
+        rel_p = ps;
+        rel_q = (qr.i + j) % p.rq;            // Q row j: step j was its last use (r = 0)
+        ++pr.i;
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int a = 0; a < NT; ++a) reg_fence(acc[a]);
+      if (wg_lead) {
+        mbar_arrive(&p_empty[rel_p]);
+        mbar_arrive(&qt_empty[rel_q]);
+        // rows j = rows .. rows + nr - 2 of the ring were loaded for the last steps and are dead now: release them
+        for (int i = rows; i < q_rows; ++i) mbar_arrive(&qt_empty[(qr.i + i) % p.rq]);
+      }
+      qr.i += q_rows;
+#pragma unroll
+      for (int a = 0; a < NT; ++a) {
+        if (a < ntaps) {
+          int r = p.r0 + a / p.ns, s = p.s0 + a % p.ns;
+          if (p.modeB) { r = p.R - 1 - r; s = p.S - 1 - s; }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int pl = 64 * wg + 16 * w4 + (lane >> 2) + 8 * h;   // P channel = accumulator row
+            if (pl < p.Pch) {
+#pragma unroll
+              for (int q = 0; q < QC / 8; ++q) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const int qc = 8 * q + 2 * (lane & 3) + e;
+                  if (qc < p.Qch) {
+                    const int k = p.modeB ? qc : pl, c = p.modeB ? pl : qc;
+                    atomicAdd(&p.dw[(((size_t)k * p.C + c) * p.R + r) * p.S + s], acc[a][4 * q + 2 * h + e]);
+                  }
+                }
               }
             }
           }
         }
       }
-      tc_fence_before();
-      mbar_arrive(tempty);
-      tph ^= 1;
     }
   }
 #undef WT_ITEM
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
-constexpr int WT_SMEM_LIMIT = 222 * 1024;
+constexpr int WT_SMEM_LIMIT = 222 * 1024;   // of H100's 227 KB per block
 constexpr int WT_SMEM_AUX = 1024 + 1024;
 inline int rup(int a, int b) { return (a + b - 1) / b * b; }
 
-template <int S>
+template <int S, int QC>
 int launch_wt(const CUtensorMap& tp, const CUtensorMap& tq, const WtParams& p, int smem, cudaStream_t st) {
-  auto kern = wgrad_tap_kernel<S>;
+  auto kern = wgrad_tap_kernel<S, QC>;
   static bool attr_set = false;
   if (!attr_set) {
     SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, WT_SMEM_LIMIT));
@@ -343,9 +328,9 @@ int launch_wt(const CUtensorMap& tp, const CUtensorMap& tq, const WtParams& p, i
   return SPC_OK;
 }
 
-// tap rectangles ("passes") of an R x S filter whose accumulators fit TMEM; returns the count (0: unsupported)
+// tap rectangles ("passes") of an R x S filter whose accumulators fit the registers; returns the count (0: unsupported)
 int plan_passes(int R, int S, int Qc16, int (*rect)[4]) {
-  const int maxt = 512 / Qc16;          // taps per pass
+  const int maxt = 128 / Qc16;          // taps per pass: the kernel's NT
   if (maxt < 1) return 0;
   int n = 0;
   if (R * S <= maxt) { rect[n][0] = 0; rect[n][1] = R; rect[n][2] = 0; rect[n][3] = S; return 1; }
@@ -392,7 +377,7 @@ int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, in
   const __nv_bfloat16* Q = p.modeB ? dy : x;
   int rect[16][4];
   const int npass = plan_passes(R, S, p.Qc16, rect);
-  SPC_REQUIRE(npass > 0, "wgrad_tap: %dx%d filter with %d Q channels does not fit TMEM", R, S, p.Qch);
+  SPC_REQUIRE(npass > 0, "wgrad_tap: %dx%d filter with %d Q channels does not fit the accumulators", R, S, p.Qch);
   CUtensorMap tp, tq;
   {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)p.Pch, (uint64_t)N};
@@ -451,12 +436,14 @@ int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, in
     p.rows_per_split = (H + best - 1) / best;
     p.num_items = base_items * best;
     const int smem = p.psn * prow + p.rq * qrow_bytes + p.rawn * rawrow + WT_SMEM_AUX;
-    int rc;
-    if (S == 1) rc = launch_wt<1>(tp, tq, p, smem, st);
-    else if (S == 3) rc = launch_wt<3>(tp, tq, p, smem, st);
-    else if (S == 5) rc = launch_wt<5>(tp, tq, p, smem, st);
-    else if (S == 7) rc = launch_wt<7>(tp, tq, p, smem, st);
-    else { set_error("wgrad_tap: unsupported filter width %d", S); return SPC_EUNSUPPORTED; }
+    int rc = SPC_EUNSUPPORTED;
+    set_error("wgrad_tap: unsupported filter width %d / %d Q channels", S, p.Qc16);
+#define WT_CASE(s, qc) if (S == s && p.Qc16 == qc) rc = launch_wt<s, qc>(tp, tq, p, smem, st);
+#define WT_CASES(s) WT_CASE(s, 16) WT_CASE(s, 32) WT_CASE(s, 48) WT_CASE(s, 64) WT_CASE(s, 80) WT_CASE(s, 96) \
+                    WT_CASE(s, 112) WT_CASE(s, 128)
+    WT_CASES(3) WT_CASES(5) WT_CASES(7)
+#undef WT_CASES
+#undef WT_CASE
     if (rc) return rc;
   }
   return SPC_OK;

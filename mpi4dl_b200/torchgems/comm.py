@@ -1,6 +1,6 @@
 """torchgems.comm -- rank arithmetic, process groups and the flat-gradient allreduce of the
 reference (src/torchgems/comm.py), re-targeted from `torch.distributed` over CUDA-aware MPI to
-one process per B200 with NCCL (gloo on CPU for the plumbing tests).
+one process per GPU with NCCL (gloo on CPU for the plumbing tests).
 
 Mirrors: initialize_cuda (comm.py:34-41), MPIComm (comm.py:44-310), sync_comms_for_master
 (comm.py:312-332), SyncAllreduce (comm.py:335-522).  Same constructor signatures, attribute names

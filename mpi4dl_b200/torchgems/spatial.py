@@ -1,5 +1,5 @@
 """torchgems.spatial -- drop-in surface of the reference's spatially-partitioned layers, backed by
-libspconv.so (hand-written sm_100a CUDA; include/spconv.h).
+libspconv.so (hand-written sm_90a CUDA; include/spconv.h).
 
 Mirrors reference src/torchgems/spatial.py:
     conv_spatial          spatial.py:25-1029   (nn.Conv2d subclass; .weight/.bias state_dict keys)
@@ -37,7 +37,7 @@ def _require_cuda(t, who):
     if not t.is_cuda:
         raise RuntimeError(
             "%s: input must be a CUDA tensor -- the spatial conv path runs only on libspconv "
-            "(sm_100a); there is no CPU fallback" % who)
+            "(sm_90a); there is no CPU fallback" % who)
 
 
 def _workspace(nbytes, device):

@@ -5,7 +5,7 @@ and the ResNet-v2-101 4096^2 spatial stage (layers_resnet101_sp2.json), at the N
 image, true zero borders on all four sides) and at the N=4 square tile (half the extent, halo
 strips PRESENT on every side the kernel shape exchanges on, i.e. an interior tile), the CUDA path
 (bf16 storage, through the C ABI) is compared -- the whole tensor, every border and every tile seam
-of the persistent tcgen05 schedule -- with what the reference computes at spatial.py:1019-1029:
+of the persistent wgmma schedule -- with what the reference computes at spatial.py:1019-1029:
 
     y      = F.conv2d(padded_tile, w, b, stride, padding=0)          cuDNN, fp32, TF32 OFF
     dx     = crop(conv2d_input(padded.shape, w, gy))                 (N2: halos are constants)
@@ -16,9 +16,10 @@ Inputs are bf16-representable, so the only differences are the fp32 summation or
 bf16 rounding of y / dx (half an ulp = 2^-9 relative).  Tolerances (written here, checked per element):
     y, dx :  |got - ref| <= 2^-7 * |ref| + 2^-8 * rms(ref)      (one bf16 ulp = 2^-8 relative, plus a floor)
     dw    :  fp32 straight from spc_conv2d_wgrad:  |got - ref| <= 1e-3 * max|ref|
-These shapes exercise num_tiles > 148 (persistent multi-tile loop, accumulator phase flips, stage-ring
-wrap), num_mg > 1 (416->1248-class M groups come from dgrad of 1664->416), wres on/off, stride 2, all
-wgrad MG variants and the multi-wave split-P schedule -- none of which the small oracle cases reach.
+These shapes exercise num_tiles > 132 (persistent multi-tile loop, stage-ring wrap), num_mg > 1
+(416->1248-class M groups come from dgrad of 1664->416), wres on/off, stride 2, all wgrad MG variants
+and the multi-wave split-P schedule -- none of which the small oracle cases reach.  The largest tensors
+(13 GB in fp32) are checked in channel slices so that every case fits an 80 GB GPU.
 """
 import ctypes as C
 import json
@@ -71,15 +72,23 @@ def _no_tf32():
 
 
 def _check(got, ref, name, rel=2.0 ** -7, floor=2.0 ** -8):
-    """per-element |got-ref| <= rel*|ref| + floor*rms(ref), whole tensor, on the device."""
+    """per-element |got-ref| <= rel*|ref| + floor*rms(ref), whole tensor, on the device (in slices of dim 1, so the
+    fp32 temporaries stay small next to the operands)."""
     assert got.shape == ref.shape, (name, tuple(got.shape), tuple(ref.shape))
-    ref = ref.float()
-    rms = float(ref.square().mean().sqrt())
+    step = max(1, (1 << 26) // max(1, ref[:, :1].numel()))
+    sq = 0.0
+    for i in range(0, ref.shape[1], step):
+        sq += float(ref[:, i:i + step].float().square().sum(dtype=torch.float64))
+    rms = (sq / ref.numel()) ** 0.5
     assert rms > 0, name
-    viol = (got.float() - ref).abs_() - (ref.abs() * rel + floor * rms)
-    worst = float(viol.max())
-    assert worst <= 0, "%s: %d elements out of tolerance, worst excess %.3g (rms %.3g)" % (
-        name, int((viol > 0).sum()), worst, rms)
+    worst, bad = float("-inf"), 0
+    for i in range(0, ref.shape[1], step):
+        r = ref[:, i:i + step].float()
+        viol = (got[:, i:i + step].float() - r).abs_() - (r.abs() * rel + floor * rms)
+        worst = max(worst, float(viol.max()))
+        bad += int((viol > 0).sum())
+        del r, viol
+    assert worst <= 0, "%s: %d elements out of tolerance, worst excess %.3g (rms %.3g)" % (name, bad, worst, rms)
 
 
 def _halo_strips(N, Cc, H, W, hh, hw, gen):
@@ -127,7 +136,7 @@ def test_conv_fullsize_vs_cudnn_fp32(case, tile):
     strips = _halo_strips(1, Cc, H, W, hh, hw, gen) if tile == "n4" else [None] * 9
     desc = (1, Cc, H, W, K, R, S, sh, sw, hh, hw, _lib.SPC_BF16, _lib.SPC_ALGO_AUTO)
     d = _lib.ConvDesc(*desc)
-    assert L.spc_conv_uses_tcgen05(C.byref(d), 0), "BASELINE shape fell off the tcgen05 path: %r" % (l,)
+    assert L.spc_conv_uses_tcgen05(C.byref(d), 0), "BASELINE shape fell off the tensor-core path: %r" % (l,)
 
     xg = x.clone().requires_grad_(not first)
     wg = w.clone().requires_grad_(True)

@@ -142,7 +142,7 @@ CONV_CASES = [
     (64, 128, (1, 1), (2, 2), 16, 32, False),
     (5, 7, (5, 5), (1, 1), 12, 12, True),
     (17, 19, (3, 3), (1, 1), 7, 5, True),         # odd everything, tile smaller than a CTA tile
-    # shapes that take the tcgen05 path in bf16 (W % 64 == 0 for multi-tap, H*W % 8 == 0 for 1x1)
+    # shapes that take the tensor-core (wgmma) path in bf16 (W % 64 == 0 for multi-tap, H*W % 8 == 0 for 1x1)
     (52, 52, (1, 7), (1, 1), 8, 128, False),
     (104, 104, (7, 1), (1, 1), 16, 64, False),
     (64, 16, (3, 3), (1, 1), 12, 192, True),
@@ -150,10 +150,10 @@ CONV_CASES = [
     (1664, 416, (1, 1), (1, 1), 8, 48, False),    # 4 M-blocks, streamed weights
     (416, 1248, (1, 1), (1, 1), 8, 32, False),    # > 512 output channels: M groups
     (104, 208, (1, 1), (2, 2), 16, 64, False),    # stride-2 pointwise (FactorizedReduce)
-    (52, 52, (3, 3), (2, 2), 32, 256, False),     # stride-2 3x3 on tcgen05 (column-subsampled copies)
+    (52, 52, (3, 3), (2, 2), 32, 256, False),     # stride-2 3x3 on wgmma (column-subsampled copies)
     (104, 104, (3, 3), (2, 2), 8, 128, False),
     (3, 104, (3, 3), (2, 2), 16, 128, False),     # the AmoebaNet stem
-    # conv_tap.cu (stride-1 taps formed in shared memory): small / partial channel boxes, odd row counts
+    # stride-1 multi-tap convolutions: small / partial channel boxes, odd row counts
     # (tile rows past the image), 5-wide filters, several 64-channel chunks, resident and streamed weights
     (3, 16, (3, 3), (1, 1), 20, 64, True),
     (16, 16, (3, 3), (1, 1), 7, 128, False),
@@ -283,7 +283,7 @@ def test_full_size_properties_linearity_and_tile_equals_slice():
     strips = [None] * 9
     strips[5] = full[:, :, :, W:W + 1].contiguous()
     y_left = conv(left, strips)
-    # interior columns come from the same (tcgen05) kernel in both runs: bit-exact.  The last
+    # interior columns come from the same (wgmma) kernel in both runs: bit-exact.  The last
     # column is recomputed by the boundary kernel from the halo strip (different fp32 summation
     # order), so it may differ by one bf16 rounding step.
     assert torch.equal(y_left[..., :W - 1], y_full[..., :W - 1])

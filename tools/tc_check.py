@@ -1,4 +1,4 @@
-"""GPU check of the tcgen05 path against a torch fp32 matmul of the same bf16 inputs (dev tool)."""
+"""GPU check of the wgmma path against a torch fp32 matmul of the same bf16 inputs (dev tool)."""
 import sys, os, time
 sys.path.insert(0, os.path.join(os.path.dirname(__file__), ".."))
 import torch
