@@ -91,7 +91,8 @@ int spc_conv2d_fwd_boundary(const spc_conv_desc* d, const void* x, const spc_hal
 
 /* dx = crop(dgrad(dy, w)) -- autograd of spatial.py:1027 followed by ZeroPad2d backward.
  * Reference semantics (SURVEY 8a N2): received halos are constants, so no gradient is sent
- * back to neighbours; dx gets only this tile's own dy contributions.  dx: [N][C][H][W]. */
+ * back to neighbours; dx gets only this tile's own dy contributions.  dx: [N][C][H][W].
+ * The opt-in exact backward adds the neighbours' part with spc_conv2d_dgrad_halo / spc_halo_accumulate below. */
 int spc_conv2d_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* dx,
                      void* workspace, size_t workspace_bytes, void* stream);
 
@@ -198,6 +199,37 @@ int spc_halo_collect_auto(void* const dst[9], const void* const src0[9], const s
                           size_t slot_bytes, spc_mailbox* self, spc_mailbox* const peers[9],
                           const int arrival_idx0[9], const int ack_idx0[9], int seq_idx, int counter_idx,
                           void* stream);
+/* ---- exact backward: the reverse halo exchange (opt-in, SPCONV_EXACT_BACKWARD=1) -------------
+ * The reference's backward treats received strips as constants (SURVEY 8a N2), so the gradient a tile's outputs
+ * owe to its neighbours' edge pixels is dropped.  The exact backward sends it back.  Strip gradient d = the part
+ * of the padded tile's input gradient that lies in pad strip d (same shapes as the received strips, but always
+ * fp32).  It travels to the neighbour in direction d, which receives it as ITS strip 8-d -- the pairing of the
+ * forward exchange -- and adds strip e into the band of real rows / columns it sent towards e (the band
+ * spc_halo_pack reads).  g[d] == NULL: no strip gradient for that direction (no neighbour there).
+ *   spc_conv2d_dgrad_halo: g[d][n][c][..] = sum_k sum_(r,s) dy[n][k][oy][ox] * w[k][c][r][s] over the output
+ *                          windows that cover the strip pixel (fp32 accumulation; any R x S, stride, dtype);
+ *   spc_pool2d_bwd_halo:   the same for pooling; x and the received strips give the max windows, which route to
+ *                          their first maximal element exactly as spc_pool2d_bwd does;
+ *   spc_halo_ring:         the pad ring of halo_exchange_layer's output gradient dy[N][C][H+2hh][W+2hw];
+ *   spc_halo_accumulate:   dx[edge band e] += g[e] for every e with g[e] != NULL: each pixel sums every strip that
+ *                          covers it (corners: row, column and corner strip) in the order e = 0..8 in fp32 and is
+ *                          rounded once to `dtype`.  No atomics: the result is bit-reproducible. */
+int spc_conv2d_dgrad_halo(const spc_conv_desc* d, const void* dy, const void* w, float* const g[9], void* stream);
+int spc_pool2d_bwd_halo(const spc_pool_desc* d, const void* x, const spc_halo* halo, const void* dy,
+                        float* const g[9], void* stream);
+int spc_halo_ring(int N, int C, int H, int W, int halo_h, int halo_w, int dtype, const void* dy, float* const g[9],
+                  void* stream);
+int spc_halo_accumulate(int N, int C, int H, int W, int halo_h, int halo_w, int dtype, void* dx,
+                        const float* const g[9], void* stream);
+/* Reverse post for the mailbox transport: spc_halo_post_auto's protocol (wait the acks of sequence s-2 of this
+ * slot, write into slot half s&1, publish s when the whole grid is done), but the payload is bytes[d] (a multiple
+ * of 4) copied from the caller's buffer src[d] to send0[d] instead of a pack of a tile.  Pair it with
+ * spc_halo_collect_auto on the same slot (its own flag block and sequence word, separate from the forward
+ * slot's), then spc_halo_accumulate.  Graph-capturable like the forward pair. */
+int spc_halo_post_strips_auto(const void* const src[9], const size_t bytes[9], void* const send0[9],
+                              size_t slot_bytes, spc_mailbox* self, spc_mailbox* const peers[9],
+                              const int ack_idx0[9], const int arrival_idx0[9], int seq_idx, int counter_idx,
+                              void* stream);
 /* After writes to peer `mb` enqueued on `stream`: publish sequence number `seq` on flag `idx`. */
 int   spc_mailbox_signal(spc_mailbox* peer_mb, int idx, uint32_t seq, void* stream);
 /* Make `stream` wait (on device) until local flag `idx` reaches `seq`. */

@@ -64,6 +64,13 @@ SYMBOLS = [
     ("spc_halo_collect_auto", C.c_int, [C.POINTER(_P * 9), C.POINTER(_P * 9), C.POINTER(C.c_size_t * 9), C.c_size_t, _P,
                                         C.POINTER(_P * 9), C.POINTER(C.c_int * 9), C.POINTER(C.c_int * 9), C.c_int, C.c_int,
                                         _P]),
+    ("spc_conv2d_dgrad_halo", C.c_int, [C.POINTER(ConvDesc), _P, _P, C.POINTER(_P * 9), _P]),
+    ("spc_pool2d_bwd_halo", C.c_int, [C.POINTER(PoolDesc), _P, C.POINTER(Halo), _P, C.POINTER(_P * 9), _P]),
+    ("spc_halo_ring", C.c_int, [C.c_int] * 7 + [_P, C.POINTER(_P * 9), _P]),
+    ("spc_halo_accumulate", C.c_int, [C.c_int] * 7 + [_P, C.POINTER(_P * 9), _P]),
+    ("spc_halo_post_strips_auto", C.c_int, [C.POINTER(_P * 9), C.POINTER(C.c_size_t * 9), C.POINTER(_P * 9), C.c_size_t,
+                                            _P, C.POINTER(_P * 9), C.POINTER(C.c_int * 9), C.POINTER(C.c_int * 9),
+                                            C.c_int, C.c_int, _P]),
     ("spc_mailbox_signal", C.c_int, [_P, C.c_int, C.c_uint32, _P]),
     ("spc_mailbox_wait", C.c_int, [_P, C.c_int, C.c_uint32, _P]),
 ]

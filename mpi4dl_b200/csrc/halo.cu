@@ -269,6 +269,24 @@ struct CollectParams {
   long long off[10];   // prefix sums of byte counts (multiples of 2)
 };
 
+// Reverse direction of the exact backward: the same protocol as halo_post_kernel, but the payload is a set of
+// caller-given (fp32) strip buffers src[d] copied into the neighbours' slots dst[d], instead of a pack of the tile.
+__global__ void halo_post_strips_kernel(const CollectParams p, const FlagSet f) {
+  const uint32_t seq = wait_flags(f);
+  const long long pofs = f.seq_word ? (long long)(seq & 1u) * f.par_bytes : 0;
+  const long long total = p.off[9] / 4;   // 4-byte units
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const long long b = i * 4;
+    int d = 0;
+#pragma unroll
+    for (int q = 1; q < 9; ++q) d += (b >= p.off[q]) ? 1 : 0;
+    const long long e = b - p.off[d];
+    *reinterpret_cast<uint32_t*>(p.dst[d] + pofs + e) = *reinterpret_cast<const uint32_t*>(p.src[d] + e);
+  }
+  signal_when_grid_done(f, seq);
+}
+
 __global__ void halo_collect_kernel(const CollectParams p, const FlagSet f) {
   const uint32_t seq = wait_flags(f);
   const long long pofs = f.seq_word ? (long long)(seq & 1u) * f.par_bytes : 0;
@@ -608,6 +626,40 @@ int spc_halo_collect_auto(void* const dst[9], const void* const src0[9], const s
               "halo_collect_auto: bad sequence / counter flag index");
   return halo_collect_impl(dst, src0, bytes, slot_bytes, self, peers, arrival_idx0, 0, ack_idx0, seq_idx, counter_idx,
                            stream);
+}
+
+int spc_halo_post_strips_auto(const void* const src[9], const size_t bytes[9], void* const send0[9], size_t slot_bytes,
+                              spc_mailbox* self, spc_mailbox* const peers[9], const int ack_idx0[9],
+                              const int arrival_idx0[9], int seq_idx, int counter_idx, void* stream) {
+  SPC_REQUIRE(src && bytes && send0 && self && peers && ack_idx0 && arrival_idx0, "halo_post_strips: null pointer");
+  SPC_REQUIRE(seq_idx >= 0 && seq_idx < self->nflags && counter_idx >= 0 && counter_idx < self->nflags,
+              "halo_post_strips_auto: bad sequence / counter flag index");
+  spc::CollectParams p{};
+  spc::FlagSet f{};
+  long long off = 0;
+  for (int d = 0; d < 9; ++d) {
+    p.off[d] = off;
+    if (d != 4 && send0[d] && bytes[d]) {
+      SPC_REQUIRE(peers[d] != nullptr && src[d] != nullptr, "halo_post_strips: missing source for direction %d", d);
+      SPC_REQUIRE(bytes[d] % 4 == 0, "halo_post_strips: strip %d is %zu bytes, not a multiple of 4", d, bytes[d]);
+      p.dst[d] = reinterpret_cast<uint8_t*>(send0[d]);
+      p.src[d] = reinterpret_cast<const uint8_t*>(src[d]);
+      off += (long long)bytes[d];
+      f.wait[d] = mb_flag(self, ack_idx0[d]);
+      f.signal[d] = mb_flag(peers[d], arrival_idx0[d]);
+    }
+  }
+  p.off[9] = off;
+  if (off == 0) return SPC_OK;
+  f.seq_word = mb_flag(self, seq_idx);
+  f.advance_seq = 0; f.wait_lag = 2; f.par_bytes = (long long)slot_bytes;
+  f.timeout_ns = spin_timeout_ns();
+  f.counter = reinterpret_cast<unsigned int*>(mb_flag(self, counter_idx));
+  const int grid = spc::grid_for((size_t)off / 4) > 64 ? 64 : spc::grid_for((size_t)off / 4);
+  spc::halo_post_strips_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p, f);
+  spc::count_launch();
+  SPC_CHECK_CUDA(cudaGetLastError());
+  return SPC_OK;
 }
 
 // ---- mailbox ---------------------------------------------------------------------------------

@@ -78,6 +78,17 @@ class DistTransport:
         exchange_strips(send, recv, ranks)
         return recv
 
+    def reverse(self, layer, grads, shape, hh, hw, mask, ranks):
+        """Reverse exchange of the exact backward: send the fp32 strip gradients grads[d] to neighbour d and return
+        the ones the neighbours send back (recv[e] belongs to this tile's edge band e).  Same pairing as exchange()."""
+        N, Cc, H, W = shape
+        recv = [None] * 9
+        for i in range(9):
+            if i != 4 and mask[i]:
+                recv[i] = torch.empty(strip_shape(i, N, Cc, H, W, hh, hw), dtype=torch.float32, device=grads[i].device)
+        exchange_strips(grads, recv, ranks)
+        return recv
+
 
 class _CudaMem:
     """Expose raw device memory to torch through __cuda_array_interface__."""
@@ -147,10 +158,12 @@ class PeerTransport:
         return ps[rank]
 
     def _slot(self, layer, x, hh, hw):
-        key = (tuple(x.shape), x.dtype, hh, hw)
+        return self._slot_for(layer, (tuple(x.shape), x.dtype, hh, hw), tuple(x.shape), x.element_size(), hh, hw)
+
+    def _slot_for(self, layer, key, shape, esize, hh, hw):
         slots = layer.__dict__.setdefault("_halo_slots", {})
         if key not in slots:
-            N, Cc, H, W = x.shape
+            N, Cc, H, W = shape
             off, offs = 0, []
             for i in range(9):
                 offs.append(off)
@@ -158,23 +171,24 @@ class PeerTransport:
                     n = 1
                     for s in strip_shape(i, N, Cc, H, W, hh, hw):
                         n *= s
-                    off += (n * x.element_size() + 255) & ~255
+                    off += (n * esize + 255) & ~255
             slot_bytes = off
             if self.data_top + 2 * slot_bytes > self.arena_bytes or self.flag_top + self.FLAGS_PER_LAYER > self.nflags:
                 raise _lib.SpconvError("halo mailbox arena exhausted; raise SPCONV_ARENA_MB")
-            slots[key] = dict(data=self.data_top, flags=self.flag_top, offs=offs, slot_bytes=slot_bytes, peer={}, plan=None)
+            slots[key] = dict(data=self.data_top, flags=self.flag_top, offs=offs, slot_bytes=slot_bytes, peer={}, plan=None,
+                              esize=esize)
             self.data_top += 2 * slot_bytes
             self.flag_top += self.FLAGS_PER_LAYER
         return slots[key]
 
-    def _plan(self, slot, x, hh, hw, mask, ranks):
+    def _plan(self, slot, shape, hh, hw, mask, ranks):
         """Argument arrays of the two protocol kernels: fixed per (layer, shape, neighbours), built once."""
         key = (tuple(mask), tuple(ranks))
         if slot["plan"] is not None and slot["plan"]["key"] == key:
             return slot["plan"]
         dirs = [i for i in range(9) if i != 4 and mask[i]]
         fb = slot["flags"]
-        N, Cc, H, W = x.shape
+        N, Cc, H, W = shape
         P9, I9, S9 = C.c_void_p * 9, C.c_int * 9, C.c_size_t * 9
         pl = dict(key=key, dirs=dirs, send=P9(), peers=P9(), src=P9(), nbytes=S9(), ack_local=I9(), arr_peer=I9(),
                   arr_local=I9(), ack_peer=I9(), shapes={})
@@ -193,7 +207,7 @@ class PeerTransport:
             for s_ in shp:
                 n *= s_
             pl["shapes"][d] = shp
-            pl["nbytes"][d] = n * x.element_size()
+            pl["nbytes"][d] = n * slot["esize"]
         slot["plan"] = pl
         return pl
 
@@ -205,7 +219,7 @@ class PeerTransport:
         L = _lib.lib()
         st = _stream()
         slot = self._slot(layer, x, hh, hw)
-        pl = self._plan(slot, x, hh, hw, mask, ranks)
+        pl = self._plan(slot, x.shape, hh, hw, mask, ranks)
         fb = slot["flags"]
         N, Cc, H, W = x.shape
         dst = (C.c_void_p * 9)()
@@ -221,6 +235,38 @@ class PeerTransport:
                                            self.mb, C.byref(pl["peers"]), C.byref(pl["arr_local"]), C.byref(pl["ack_peer"]),
                                            fb + self._SEQ, fb + self._CNT_COLLECT, st), "spc_halo_collect_auto")
         return recv
+
+    def reverse(self, layer, grads, shape, hh, hw, mask, ranks):
+        """Reverse exchange of the exact backward (see DistTransport.reverse).  The layer gets a second slot for it,
+        fp32-sized, with its own flag block and sequence word, so forward and reverse exchanges of one layer may
+        interleave freely; its offsets are swapped with each neighbour at first use like the forward slot's.
+        spc_halo_post_strips_auto copies grads[d] into neighbour d's reverse slot, spc_halo_collect_auto copies
+        what the neighbours wrote out of this rank's.  Graph-capturable like exchange()."""
+        L = _lib.lib()
+        st = _stream()
+        shape = tuple(shape)
+        slot = self._slot_for(layer, ("reverse", shape, hh, hw), shape, 4, hh, hw)
+        pl = self._plan(slot, shape, hh, hw, mask, ranks)
+        fb = slot["flags"]
+        src = (C.c_void_p * 9)()
+        dst = (C.c_void_p * 9)()
+        recv = [None] * 9
+        for d in pl["dirs"]:
+            src[d] = grads[d].data_ptr()
+            recv[d] = torch.empty(pl["shapes"][d], dtype=torch.float32, device=grads[d].device)
+            dst[d] = recv[d].data_ptr()
+        _lib.check(L.spc_halo_post_strips_auto(C.byref(src), C.byref(pl["nbytes"]), C.byref(pl["send"]), slot["slot_bytes"],
+                                               self.mb, C.byref(pl["peers"]), C.byref(pl["ack_local"]),
+                                               C.byref(pl["arr_peer"]), fb + self._SEQ, fb + self._CNT_POST, st),
+                   "spc_halo_post_strips_auto")
+        _lib.check(L.spc_halo_collect_auto(C.byref(dst), C.byref(pl["src"]), C.byref(pl["nbytes"]), slot["slot_bytes"],
+                                           self.mb, C.byref(pl["peers"]), C.byref(pl["arr_local"]), C.byref(pl["ack_peer"]),
+                                           fb + self._SEQ, fb + self._CNT_COLLECT, st), "spc_halo_collect_auto")
+        return recv
+
+    def arena_high_water(self):
+        """Bytes of the mailbox arena handed out to slots so far."""
+        return self.data_top
 
 
 _transport = None
@@ -299,6 +345,12 @@ def get_transport(device):
 def overlap_enabled():
     """Overlap the exchange (comm stream) with the interior pass; SPCONV_HALO_OVERLAP=0 serialises."""
     return os.environ.get("SPCONV_HALO_OVERLAP", "1") != "0"
+
+
+def exact_backward_default():
+    """Initial value of a spatial layer's `exact_backward`: SPCONV_EXACT_BACKWARD=1 sends the gradients of the
+    received halo strips back to the neighbours, so that the tiles' input gradients equal the unsplit image's."""
+    return os.environ.get("SPCONV_EXACT_BACKWARD", "0") == "1"
 
 
 def set_transport(t):

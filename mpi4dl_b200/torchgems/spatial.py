@@ -172,20 +172,70 @@ def _comm_stream(device):
     return _comm_streams[key]
 
 
+def _alloc_strip_grads(mask, N, Cc, H, W, hh, hw, device):
+    """fp32 buffers for the gradients of the received strips (None where there is no neighbour)."""
+    return [torch.empty(_strip_shape(i, N, Cc, H, W, hh, hw), dtype=torch.float32, device=device)
+            if (i != 4 and mask[i]) else None for i in range(9)]
+
+
+def _strip_ptrs(strips):
+    return (C.c_void_p * 9)(*[C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(None) for t in strips])
+
+
+def _reverse_begin(layer, grads, shape, hh, hw):
+    """Start the reverse halo exchange of the exact backward: send the strip gradients `grads` to the neighbours.
+    Returns (received strip gradients, event that fires when they have arrived, or None).  With
+    SPCONV_HALO_OVERLAP on, the exchange runs on the comm stream while the caller's dgrad / wgrad run on this one.
+    Every rank enqueues its reverse exchanges in the order autograd runs the backward functions.  Nothing makes
+    the ranks agree on that order except that every tile builds the same module tree and runs the same forward,
+    so their autograd graphs are identical; a rank that took a different path would wait on a neighbour's slot
+    that never fills (the spin bound, SPCONV_SPIN_TIMEOUT_S, turns that into an error)."""
+    tr = halo_transport.get_transport(grads[[i for i in range(9) if grads[i] is not None][0]].device)
+    if not halo_transport.overlap_enabled():
+        return tr.reverse(layer, grads, shape, hh, hw, layer.neighbours, layer.rank_neighbours), None
+    main = torch.cuda.current_stream()
+    comm = _comm_stream(main.device)
+    comm.wait_stream(main)                             # the strip gradients are complete
+    with torch.cuda.stream(comm):
+        recv = tr.reverse(layer, grads, shape, hh, hw, layer.neighbours, layer.rank_neighbours)
+        ready = torch.cuda.Event()
+        ready.record(comm)
+    for t in grads:
+        if t is not None:
+            t.record_stream(comm)
+    for t in recv:
+        if t is not None:
+            t.record_stream(main)
+    return recv, ready
+
+
+def _reverse_finish(recv, ready, dx, hh, hw):
+    """dx[edge bands] += the strip gradients the neighbours sent back."""
+    if ready is not None:
+        torch.cuda.current_stream().wait_event(ready)
+    N, Cc, H, W = dx.shape
+    _lib.check(_lib.lib().spc_halo_accumulate(N, Cc, H, W, hh, hw, _lib.dtype_code(dx.dtype), _ptr(dx),
+                                              C.byref(_strip_ptrs(recv)), _stream()), "spc_halo_accumulate")
+
+
 class _ConvSpatialFn(torch.autograd.Function):
-    """fprop / dgrad / wgrad through the C ABI.  Halo strips enter as constants: the reference
-    unpacks them with in-place slice assignment of detached tensors, so no gradient ever flows
-    back to a neighbour (SURVEY 8a N2)."""
+    """fprop / dgrad / wgrad through the C ABI.  By default halo strips enter as constants: the
+    reference unpacks them with in-place slice assignment of detached tensors, so no gradient ever
+    flows back to a neighbour (SURVEY 8a N2).  Given the layer (exact backward), the gradient of
+    the received strips is sent back and added into the neighbours' dx."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, desc_args, *strips):
         """strips[0:9] are the received halo strips; an optional 10th element is a CUDA event that
         fires when they have arrived (exchange running on the comm stream): then the interior pass
-        is launched first and only the boundary strips wait for the event."""
+        is launched first and only the boundary strips wait for the event.  An optional 11th element
+        is the conv_spatial layer whose strips they are: backward then runs the reverse exchange
+        (exact backward) with the layer's neighbours and transport slots."""
         L = _lib.lib()
         d = _lib.ConvDesc(*desc_args)
         ctx.n_tail = len(strips)
         ready = strips[9] if len(strips) > 9 else None
+        ctx.layer = strips[10] if len(strips) > 10 else None
         strips = strips[:9]
         Ho, Wo = C.c_int(), C.c_int()
         L.spc_conv_out_shape(C.byref(d), C.byref(Ho), C.byref(Wo))
@@ -217,6 +267,14 @@ class _ConvSpatialFn(torch.autograd.Function):
         d = _lib.ConvDesc(*ctx.desc_args)
         gy = gy.contiguous()
         dx = dw = db = None
+        # exact backward: strip gradients (need only gy, w) -> reverse exchange on the comm stream, under dgrad and
+        # wgrad on this one -> accumulate.  Skipped when x needs no gradient (the same decision on every rank).
+        exact = ctx.layer is not None and ctx.needs_input_grad[0]
+        if exact:
+            grads = _alloc_strip_grads(ctx.layer.neighbours, d.N, d.C, d.H, d.W, d.pad_h, d.pad_w, x.device)
+            _lib.check(L.spc_conv2d_dgrad_halo(C.byref(d), _ptr(gy), _ptr(weight), C.byref(_strip_ptrs(grads)), _stream()),
+                       "spc_conv2d_dgrad_halo")
+            recv, ready = _reverse_begin(ctx.layer, grads, x.shape, d.pad_h, d.pad_w)
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)
             ws, wsp = _workspace(L.spc_conv_workspace_bytes(C.byref(d), 1), x.device)
@@ -231,6 +289,8 @@ class _ConvSpatialFn(torch.autograd.Function):
                                           wsp, 0 if ws is None else ws.numel(), _stream()), "spc_conv2d_wgrad")
             dw = dw32.to(weight.dtype)
             db = db32.to(weight.dtype) if db32 is not None else None
+        if exact:
+            _reverse_finish(recv, ready, dx, d.pad_h, d.pad_w)
         return (dx, dw, db, None) + (None,) * ctx.n_tail
 
 
@@ -285,6 +345,8 @@ class conv_spatial(nn.Conv2d, _SpatialTopology):
             self.neighbours = None          # never exchanges
         self.set_tags()
         self.algo = _lib.SPC_ALGO_AUTO
+        # a plain attribute (not a parameter / buffer: state_dict keys stay the reference's), flippable per layer
+        self.exact_backward = halo_transport.exact_backward_default()
 
     def _fused_pre(self, x):
         """D2 variant, strided: a side that faces a neighbour carries NO padding, so the sampling phase of a strided
@@ -348,6 +410,8 @@ class conv_spatial(nn.Conv2d, _SpatialTopology):
                 extra = (ready,)
             else:
                 strips = self._exchange(x, hh, hw) if exchange else [None] * 9
+        if exchange and self.exact_backward:
+            extra = (extra[0] if extra else None, self)
         y = _ConvSpatialFn.apply(x, self.weight, self.bias, desc_args, *strips, *extra)
         if self.fused_halo:
             y = self._crop_fused(y, H0, W0, et, el)
@@ -357,7 +421,12 @@ class conv_spatial(nn.Conv2d, _SpatialTopology):
 class _HaloPadFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, halo_len, *strips):
+        """strips[0:9]: the received strips; an optional 10th element is the halo_exchange_layer (exact backward:
+        the pad ring of the output gradient is sent back to the neighbours)."""
         L = _lib.lib()
+        ctx.n_tail = len(strips)
+        ctx.layer = strips[9] if len(strips) > 9 else None
+        strips = strips[:9]
         N, Cc, H, W = x.shape
         y = torch.empty((N, Cc, H + 2 * halo_len, W + 2 * halo_len), dtype=x.dtype, device=x.device)
         halo = _lib.make_halo(strips)
@@ -371,11 +440,20 @@ class _HaloPadFn(torch.autograd.Function):
     def backward(ctx, gy):
         L = _lib.lib()
         N, Cc, H, W = ctx.shape
+        h = ctx.halo_len
         gy = gy.contiguous()
+        exact = ctx.layer is not None and ctx.needs_input_grad[0]
+        if exact:
+            grads = _alloc_strip_grads(ctx.layer.neighbours, N, Cc, H, W, h, h, gy.device)
+            _lib.check(L.spc_halo_ring(N, Cc, H, W, h, h, _lib.dtype_code(gy.dtype), _ptr(gy), C.byref(_strip_ptrs(grads)),
+                                       _stream()), "spc_halo_ring")
+            recv, ready = _reverse_begin(ctx.layer, grads, ctx.shape, h, h)
         dx = torch.empty(ctx.shape, dtype=gy.dtype, device=gy.device)
-        _lib.check(L.spc_halo_crop(N, Cc, H, W, ctx.halo_len, ctx.halo_len, _lib.dtype_code(gy.dtype), _ptr(gy),
+        _lib.check(L.spc_halo_crop(N, Cc, H, W, h, h, _lib.dtype_code(gy.dtype), _ptr(gy),
                                    _ptr(dx), _stream()), "spc_halo_crop")
-        return (dx, None) + (None,) * 9
+        if exact:
+            _reverse_finish(recv, ready, dx, h, h)
+        return (dx, None) + (None,) * ctx.n_tail
 
 
 class halo_exchange_layer(nn.Module, _SpatialTopology):
@@ -391,20 +469,26 @@ class halo_exchange_layer(nn.Module, _SpatialTopology):
         if self.neighbours is not None:
             self.get_neighbours_rank()
         self.set_tags()
+        self.exact_backward = halo_transport.exact_backward_default()
 
     def forward(self, tensor):
         _require_cuda(tensor, "halo_exchange_layer")
         x = tensor.contiguous()
         with torch.no_grad():
             strips = self._exchange(x, self.halo_len, self.halo_len) if self.halo_len > 0 else [None] * 9
-        return _HaloPadFn.apply(x, self.halo_len, *strips)
+        tail = (self,) if self.exact_backward and any(s is not None for s in strips) else ()
+        return _HaloPadFn.apply(x, self.halo_len, *strips, *tail)
 
 
 class _PoolFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, desc_args, *strips):
+        """strips[0:9]: the received strips; an optional 10th element is the Pool layer (exact backward)."""
         L = _lib.lib()
         d = _lib.PoolDesc(*desc_args)
+        ctx.n_tail = len(strips)
+        ctx.layer = strips[9] if len(strips) > 9 else None
+        strips = strips[:9]
         Ho = (d.H + 2 * d.pad - d.k) // d.stride + 1
         Wo = (d.W + 2 * d.pad - d.k) // d.stride + 1
         y = torch.empty((d.N, d.C, Ho, Wo), dtype=x.dtype, device=x.device)
@@ -424,11 +508,19 @@ class _PoolFn(torch.autograd.Function):
         strips = [next(it) if m else None for m in ctx.strip_mask]
         d = _lib.PoolDesc(*ctx.desc_args)
         gy = gy.contiguous()
-        dx = torch.empty_like(x)
         halo = _lib.make_halo(strips)
+        exact = ctx.layer is not None and ctx.needs_input_grad[0]
+        if exact:
+            grads = _alloc_strip_grads(ctx.layer.neighbours, d.N, d.C, d.H, d.W, d.pad, d.pad, x.device)
+            _lib.check(L.spc_pool2d_bwd_halo(C.byref(d), _ptr(x), C.byref(halo), _ptr(gy), C.byref(_strip_ptrs(grads)),
+                                             _stream()), "spc_pool2d_bwd_halo")
+            recv, ready = _reverse_begin(ctx.layer, grads, x.shape, d.pad, d.pad)
+        dx = torch.empty_like(x)
         _lib.check(L.spc_pool2d_bwd(C.byref(d), _ptr(x), C.byref(halo), _ptr(gy), _ptr(dx), _stream()),
                    "spc_pool2d_bwd")
-        return (dx, None) + (None,) * 9
+        if exact:
+            _reverse_finish(recv, ready, dx, d.pad, d.pad)
+        return (dx, None) + (None,) * ctx.n_tail
 
 
 class Pool(nn.Module, _SpatialTopology):
@@ -468,6 +560,7 @@ class Pool(nn.Module, _SpatialTopology):
             if self.neighbours is not None:
                 self.get_neighbours_rank()
         self.set_tags()
+        self.exact_backward = halo_transport.exact_backward_default()
 
     def forward(self, tensor):
         _require_cuda(tensor, "Pool")
@@ -478,7 +571,8 @@ class Pool(nn.Module, _SpatialTopology):
         mode = _lib.SPC_POOL_MAX if self.operation == "MaxPool2d" else _lib.SPC_POOL_AVG
         desc_args = (N, Cc, H, W, self.kernel_size[0], self.stride[0], self.halo_len, mode,
                      _lib.dtype_code(x.dtype))
-        return _PoolFn.apply(x, desc_args, *strips)
+        tail = (self,) if self.exact_backward and any(s is not None for s in strips) else ()
+        return _PoolFn.apply(x, desc_args, *strips, *tail)
 
 
 class local_conv2d(nn.Conv2d):
