@@ -2,12 +2,11 @@
 //
 // Dispatch: shapes the wgmma implicit-GEMM path supports (gemm_tc.cu) run there over the
 // whole tile with zero padding; if the tile has neighbours, the thin output strips whose
-// receptive field reaches into a halo are then recomputed by the direct kernel, which reads the
-// received strips in place.  Interior compute therefore never waits on the halo exchange --
-// the overlap the reference left as dead code (spatial.py:415-866).  Everything else runs
-// entirely on the direct kernel.
-#include <stdlib.h>
-
+// receptive field reaches into a halo are then recomputed by a small GEMM over just those
+// outputs, which reads the received strips in place.  Interior compute therefore never waits on
+// the halo exchange -- the overlap the reference left as dead code (spatial.py:415-866).
+// Everything else runs entirely on the direct kernel; when its interior and boundary passes are
+// split (spc_conv2d_fwd_interior / _boundary, fp32 or SPC_ALGO_DIRECT), it recomputes the strips.
 #include "common.cuh"
 
 namespace spc {
@@ -49,73 +48,12 @@ DirectConvParams fwd_params(const spc_conv_desc* d, const void* x, const spc_hal
 
 inline size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
 
-// Boundary rect through the tensor-core path: gather a 64-column-aligned patch of tile+halo around the
-// rect, run the SAME fast convolution on that small image, scatter the rect back.  Stride 1 only.
-static bool patch_ok(const spc_conv_desc* d, int op) {
-  if (d->dtype != SPC_BF16 || d->stride_h != 1 || d->stride_w != 1 || d->algo == SPC_ALGO_DIRECT) return false;
-  spc_conv_desc q = *d;
-  q.H = 64; q.W = 64; q.N = d->N;
-  return tc_supported(&q, op);
-}
-
-static int patch_fwd_rect(const spc_conv_desc* d, const void* x, const spc_halo* halo, const void* w, const void* bias,
-                          void* y, int y0, int y1, int x0, int x1, cudaStream_t st) {
-  if (y1 <= y0 || x1 <= x0) return SPC_OK;
-  const int rh = y1 - y0, rw = x1 - x0, ph = d->pad_h, pw = d->pad_w;
-  spc_conv_desc q = *d;
-  q.H = rh + 2 * ph;
-  q.W = ((rw + 2 * pw) + 63) & ~63;
-  q.algo = SPC_ALGO_TCGEN05;
-  const size_t esz = dtype_size(d->dtype);
-  const size_t pbytes = al256((size_t)d->N * d->C * q.H * q.W * esz), obytes = al256((size_t)d->N * d->K * q.H * q.W * esz);
-  const size_t wsb = tc_workspace_bytes(&q, 0);
-  char* base = (char*)boundary_scratch(pbytes + obytes + wsb + 1024);
-  SPC_REQUIRE(base != nullptr, "boundary scratch allocation failed");
-  void* P = base; void* O = base + pbytes; void* ws = base + pbytes + obytes;
-  TileView v = make_view(x, halo, d->N, d->C, d->H, d->W, ph, pw);
-  int rc = launch_patch_gather(v, P, q.H, q.W, y0 - ph, x0 - pw, d->dtype, st);
-  if (rc) return rc;
-  rc = tc_conv_fwd(&q, P, w, bias, O, ws, wsb, st);
-  if (rc) return rc;
-  int Ho, Wo;
-  spc_conv_out_shape(d, &Ho, &Wo);
-  return launch_patch_scatter(O, y, d->N * d->K, Ho, Wo, q.H, q.W, y0, x0, rh, rw, ph, pw, d->dtype, st);
-}
-
-// dw += (halo pixels only) x (dy restricted to the rect), through the wgmma wgrad on a patch
-static int patch_wgrad_rect(const spc_conv_desc* d, const spc_halo* halo, const void* dy, float* dw, int y0, int y1,
-                            int x0, int x1, cudaStream_t st) {
-  if (y1 <= y0 || x1 <= x0) return SPC_OK;
-  const int rh = y1 - y0, rw = x1 - x0, ph = d->pad_h, pw = d->pad_w;
-  spc_conv_desc q = *d;
-  q.H = rh + 2 * ph;
-  q.W = ((rw + 2 * pw) + 63) & ~63;
-  q.algo = SPC_ALGO_TCGEN05;
-  const size_t esz = dtype_size(d->dtype);
-  const size_t pbytes = al256((size_t)d->N * d->C * q.H * q.W * esz), gbytes = al256((size_t)d->N * d->K * q.H * q.W * esz);
-  const size_t wsb = tc_workspace_bytes(&q, 2);
-  char* base = (char*)boundary_scratch(pbytes + gbytes + wsb + 1024);
-  SPC_REQUIRE(base != nullptr, "boundary scratch allocation failed");
-  void* P = base; void* G = base + pbytes; void* ws = base + pbytes + gbytes;
-  TileView v = make_view(nullptr, halo, d->N, d->C, d->H, d->W, ph, pw);   // halo pixels only
-  int rc = launch_patch_gather(v, P, q.H, q.W, y0 - ph, x0 - pw, d->dtype, st);
-  if (rc) return rc;
-  int Ho, Wo;
-  spc_conv_out_shape(d, &Ho, &Wo);
-  rc = launch_patch_gather_dy(dy, G, d->N * d->K, Ho, Wo, q.H, q.W, y0, x0, rh, rw, ph, pw, d->dtype, st);
-  if (rc) return rc;
-  return tc_conv_wgrad(&q, P, G, dw, 1, ws, wsb, st);
-}
-
 // ---- halo fix-up of the tensor-core paths: a small GEMM over the boundary outputs only ------------------------------
 // After the interior pass ran the whole tile with zero padding, only the outputs whose window reaches a received
 // strip are wrong (P_b of them: a few rows / columns).  fprop: V[(c,r,s)][p] = im2col of tile + strips over those
 // P_b outputs, then ONE pointwise GEMM  O[K][P_b] = w[K][C*R*S] * V (+bias)  on the wgmma kernel -- the filter tensor
 // IS that matrix -- and a scatter that overwrites them.  wgrad: the halo pixels' share is linear, so with V taken
 // from the HALO-ONLY view  dW[K][C*R*S] += dY_b[K][P_b] * V^T  (pw_wgrad_kernel accumulating straight into dw).
-// The alternative (SPC_BOUNDARY_V1=1) gathers a 64-column-aligned patch around every boundary rectangle and re-runs the
-// convolution on it: 3 launches per rectangle, up to 4 rectangles, and strided layers fall to the direct kernel on thin
-// strips -- on small tiles that can cost more than the interior pass itself.
 static bool boundary_rects(const spc_conv_desc* d, const spc_halo* halo, int Ho, int Wo, BoundaryRects* b) {
   const int top = min(Ho, ceil_div(d->pad_h, d->stride_h));
   int bot0 = ceil_div(d->H + d->pad_h - d->R + 1, d->stride_h);      // first output row touching the bottom halo
@@ -221,36 +159,17 @@ size_t spc_conv_workspace_bytes(const spc_conv_desc* d, int op) {
 }
 
 // Boundary strips: output rows / columns whose window reaches outside the tile, recomputed from
-// tile + received halo strips (direct kernel).  Valid after ANY interior pass that used zero padding.
+// tile + received halo strips.  Valid after ANY interior pass that used zero padding.
 static int fwd_boundary(const spc_conv_desc* d, DirectConvParams p, const spc_halo* halo, cudaStream_t st) {
   if (!has_halo(halo)) return SPC_OK;
-  int rc;
-  const int Ho = p.Ho, Wo = p.Wo;
-  const int top = min(Ho, ceil_div(d->pad_h, d->stride_h));
-  int bot0 = ceil_div(d->H + d->pad_h - d->R + 1, d->stride_h);  // first row touching the bottom halo
-  bot0 = max(top, min(Ho, bot0));
-  const int left = min(Wo, ceil_div(d->pad_w, d->stride_w));
-  int right0 = ceil_div(d->W + d->pad_w - d->S + 1, d->stride_w);
-  right0 = max(left, min(Wo, right0));
-  const bool any_top = halo->strip[0] || halo->strip[1] || halo->strip[2];
-  const bool any_bot = halo->strip[6] || halo->strip[7] || halo->strip[8];
-  const bool any_left = halo->strip[0] || halo->strip[3] || halo->strip[6];
-  const bool any_right = halo->strip[2] || halo->strip[5] || halo->strip[8];
-  const int sy0 = any_top ? top : 0, sy1 = any_bot ? bot0 : Ho;   // rows not already redone by the bands
-  if (d->dtype == SPC_BF16 && d->algo != SPC_ALGO_DIRECT && !getenv("SPC_BOUNDARY_V1"))
-    return boundary_fwd_tc(d, p.in.x, halo, p.w, p.bias, p.y, st);
-  if (patch_ok(d, 0)) {
-    const void* x = p.in.x; const void* w = p.w; const void* bias = p.bias; void* y = p.y;
-    if (any_top && (rc = patch_fwd_rect(d, x, halo, w, bias, y, 0, top, 0, Wo, st))) return rc;
-    if (any_bot && (rc = patch_fwd_rect(d, x, halo, w, bias, y, bot0, Ho, 0, Wo, st))) return rc;
-    if (any_left && (rc = patch_fwd_rect(d, x, halo, w, bias, y, sy0, sy1, 0, left, st))) return rc;
-    if (any_right && (rc = patch_fwd_rect(d, x, halo, w, bias, y, sy0, sy1, right0, Wo, st))) return rc;
-    return SPC_OK;
+  if (d->dtype == SPC_BF16 && d->algo != SPC_ALGO_DIRECT) return boundary_fwd_tc(d, p.in.x, halo, p.w, p.bias, p.y, st);
+  // fp32 and SPC_ALGO_DIRECT: the direct kernel on each boundary rectangle
+  BoundaryRects b;
+  if (!boundary_rects(d, halo, p.Ho, p.Wo, &b)) return SPC_OK;
+  for (int i = 0; i < b.n; ++i) {
+    const int rc = fwd_rect(p, d->dtype, b.y0[i], b.y1[i], b.x0[i], b.x1[i], st);
+    if (rc) return rc;
   }
-  if (any_top && (rc = fwd_rect(p, d->dtype, 0, top, 0, Wo, st))) return rc;
-  if (any_bot && (rc = fwd_rect(p, d->dtype, bot0, Ho, 0, Wo, st))) return rc;
-  if (any_left && (rc = fwd_rect(p, d->dtype, sy0, sy1, 0, left, st))) return rc;
-  if (any_right && (rc = fwd_rect(p, d->dtype, sy0, sy1, right0, Wo, st))) return rc;
   return SPC_OK;
 }
 
@@ -369,40 +288,20 @@ int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo
     set_error("conv_wgrad: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
     return SPC_EUNSUPPORTED;
   }
-  DirectWgradParams p{};
-  p.dy = dy; p.dw = dw;
-  p.K = d->K; p.R = d->R; p.S = d->S; p.sh = d->stride_h; p.sw = d->stride_w; p.ph = d->pad_h; p.pw = d->pad_w;
-  p.Ho = Ho; p.Wo = Wo;
   if (tc) {
     rc = tc_conv_wgrad(d, x, dy, dw, /*accumulate=*/1, workspace, workspace_bytes, st);
     if (rc) return rc;
+    // add the halo pixels' contribution (exact by linearity): boundary GEMM over the outputs whose windows reach a strip
     if (has_halo(halo)) {
-      // add the halo pixels' contribution: the direct kernel over a view that holds ONLY the
-      // strips (interior reads as zero) -- exact by linearity -- restricted to the output strips
-      // whose windows reach outside the tile.
-      if (d->dtype == SPC_BF16 && !getenv("SPC_BOUNDARY_V1")) {
-        rc = boundary_wgrad_tc(d, halo, dy, dw, st);
-        if (rc) return rc;
-      } else if (patch_ok(d, 2)) {
-        const int top = min(Ho, d->pad_h), bot0 = max(top, min(Ho, d->H + d->pad_h - d->R + 1));
-        const int left = min(Wo, d->pad_w), right0 = max(left, min(Wo, d->W + d->pad_w - d->S + 1));
-        const bool any_top = halo->strip[0] || halo->strip[1] || halo->strip[2];
-        const bool any_bot = halo->strip[6] || halo->strip[7] || halo->strip[8];
-        const bool any_left = halo->strip[0] || halo->strip[3] || halo->strip[6];
-        const bool any_right = halo->strip[2] || halo->strip[5] || halo->strip[8];
-        const int sy0 = any_top ? top : 0, sy1 = any_bot ? bot0 : Ho;
-        if (any_top && (rc = patch_wgrad_rect(d, halo, dy, dw, 0, top, 0, Wo, st))) return rc;
-        if (any_bot && (rc = patch_wgrad_rect(d, halo, dy, dw, bot0, Ho, 0, Wo, st))) return rc;
-        if (any_left && (rc = patch_wgrad_rect(d, halo, dy, dw, sy0, sy1, 0, left, st))) return rc;
-        if (any_right && (rc = patch_wgrad_rect(d, halo, dy, dw, sy0, sy1, right0, Wo, st))) return rc;
-      } else {
-        p.in = make_view(nullptr, halo, d->N, d->C, d->H, d->W, d->pad_h, d->pad_w);
-        rc = launch_wgrad_halo(p, d->dtype, st);
-        if (rc) return rc;
-      }
+      rc = boundary_wgrad_tc(d, halo, dy, dw, st);
+      if (rc) return rc;
     }
   } else {
+    DirectWgradParams p{};
     p.in = make_view(x, halo, d->N, d->C, d->H, d->W, d->pad_h, d->pad_w);
+    p.dy = dy; p.dw = dw;
+    p.K = d->K; p.R = d->R; p.S = d->S; p.sh = d->stride_h; p.sw = d->stride_w; p.ph = d->pad_h; p.pw = d->pad_w;
+    p.Ho = Ho; p.Wo = Wo;
     rc = launch_wgrad_direct(p, d->dtype, st);
     if (rc) return rc;
   }

@@ -128,19 +128,10 @@ struct DirectWgradParams {
   int ry0, rx0, rH, rW;   // output sub-rectangle to reduce over (rH == 0: the whole output)
 };
 int launch_wgrad_direct(const DirectWgradParams& p, int dtype, cudaStream_t st);
-// dw += contribution of the halo pixels only (boundary output pixels x taps that fall outside the tile)
-int launch_wgrad_halo(const DirectWgradParams& p, int dtype, cudaStream_t st);
 int launch_bias_grad(const void* dy, float* db, int N, int K, int HW, int dtype, int accumulate, cudaStream_t st);
 
-// ---- boundary patches (halo.cu) ---------------------------------------------------------------
-void* boundary_scratch(size_t bytes);
-int launch_patch_gather(const TileView& v, void* P, int Hp, int Wp, int h0, int w0, int dtype, cudaStream_t st);
-int launch_patch_gather_dy(const void* dy, void* G, int NK, int Ho, int Wo, int Hp, int Wp, int y0, int x0, int rh, int rw,
-                           int ph, int pw, int dtype, cudaStream_t st);
-int launch_patch_scatter(const void* O, void* y, int NK, int Ho, int Wo, int Hp, int Wp, int y0, int x0, int rh, int rw,
-                         int ph, int pw, int dtype, cudaStream_t st);
-
 // ---- halo fix-up as a small GEMM over the boundary outputs only (halo.cu kernels, api.cu orchestration) ----------
+void* boundary_scratch(size_t bytes);   // grow-only device scratch of the fix-up's operands
 // The boundary outputs of a tile (those whose window reaches a received strip) are listed as <= 4 disjoint output
 // rectangles; P_b = their pixel count (x N), padded to a multiple of 64.
 struct BoundaryRects {

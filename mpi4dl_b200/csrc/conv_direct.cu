@@ -289,93 +289,6 @@ int launch_conv_direct(const DirectConvParams& p, int dtype, cudaStream_t st) {
   return SPC_OK;
 }
 
-// ---------------------------------------------------------------------------------------------
-// Halo-only wgrad correction: dw[k][c][tap] += sum over boundary output pixels p and taps whose
-// input pixel lies OUTSIDE the tile of dy[k][p] * halo(c, pixel).  One thread per (k, c) pair of a
-// 16 x 16 block; blockIdx.y walks chunks of the boundary-pixel list; whether a (pixel, tap) pair is
-// outside is uniform across the block, so there is no divergence.
-constexpr int WH_TG = 8;   // taps per register pass
-template <typename T>
-__global__ void __launch_bounds__(256)
-wgrad_halo_kernel(const DirectWgradParams p, const int kblocks, const int npix, const int pix_per_cta, const int top,
-                  const int bot0, const int left, const int right0) {
-  const int kb = blockIdx.x % kblocks, cb = blockIdx.x / kblocks;
-  const int k = kb * 16 + threadIdx.x / 16, c = cb * 16 + threadIdx.x % 16;
-  const int C = p.in.C, taps = p.R * p.S;
-  const bool active = k < p.K && c < C;
-  const T* dy = reinterpret_cast<const T*>(p.dy);
-  // boundary pixel list = top band rows [0,top) | bottom band [bot0,Ho) | left cols | right cols (middle rows)
-  const int n_top = top * p.Wo, n_bot = (p.Ho - bot0) * p.Wo, mid = bot0 - top;
-  const int n_left = mid * left, wr = p.Wo - right0;
-  const int per_image = n_top + n_bot + n_left + mid * wr;
-  const int q0 = blockIdx.y * pix_per_cta, q1 = min(npix, q0 + pix_per_cta);
-  for (int tg = 0; tg < taps; tg += WH_TG) {
-    const int r_first = tg / p.S, s_first = tg % p.S;
-    float acc[WH_TG];
-#pragma unroll
-    for (int u = 0; u < WH_TG; ++u) acc[u] = 0.f;
-    for (int q = q0; q < q1; ++q) {
-      const int n = q / per_image;
-      int e = q - n * per_image, oy, ox;
-      if (e < n_top) { oy = e / p.Wo; ox = e - oy * p.Wo; }
-      else if ((e -= n_top) < n_bot) { oy = e / p.Wo; ox = e - oy * p.Wo; oy += bot0; }
-      else if ((e -= n_bot) < n_left) { oy = e / left; ox = e - oy * left; oy += top; }
-      else { e -= n_left; oy = e / wr; ox = right0 + e - oy * wr; oy += top; }
-      const int h0 = oy * p.sh - p.ph, w0 = ox * p.sw - p.pw;
-      // does any tap of this pass fall outside the tile? (block-uniform)  rows h0+r, cols w0+s
-      float g = 0.f;
-      bool loaded = false;
-      int r = r_first, sx = s_first;
-#pragma unroll
-      for (int u = 0; u < WH_TG; ++u) {
-        if (tg + u < taps) {
-          const int h = h0 + r, w = w0 + sx;
-          if ((unsigned)h >= (unsigned)p.in.H || (unsigned)w >= (unsigned)p.in.W) {
-            if (!loaded) {
-              g = active ? to_f32<T>(dy[(((size_t)n * p.K + k) * p.Ho + oy) * p.Wo + ox]) : 0.f;
-              loaded = true;
-            }
-            if (active) {
-              const T* ptr = tile_ptr<T>(p.in, n, c, h, w);
-              if (ptr) acc[u] = fmaf(g, to_f32<T>(__ldg(ptr)), acc[u]);
-            }
-          }
-          if (++sx == p.S) { sx = 0; ++r; }
-        }
-      }
-    }
-    if (active) {
-#pragma unroll
-      for (int u = 0; u < WH_TG; ++u)
-        if (tg + u < taps && acc[u] != 0.f) atomicAdd(&p.dw[((size_t)k * C + c) * taps + tg + u], acc[u]);
-    }
-  }
-}
-
-int launch_wgrad_halo(const DirectWgradParams& p, int dtype, cudaStream_t st) {
-  const int top = min(p.Ho, ceil_div(p.ph, p.sh));
-  const int bot0 = max(top, min(p.Ho, ceil_div(p.in.H + p.ph - p.R + 1, p.sh)));
-  const int left = min(p.Wo, ceil_div(p.pw, p.sw));
-  const int right0 = max(left, min(p.Wo, ceil_div(p.in.W + p.pw - p.S + 1, p.sw)));
-  const int per_image = top * p.Wo + (p.Ho - bot0) * p.Wo + (bot0 - top) * (left + p.Wo - right0);
-  const long long npix = (long long)per_image * p.in.N;
-  if (npix <= 0) return SPC_OK;
-  const int kblocks = ceil_div(p.K, 16), cblocks = ceil_div(p.in.C, 16);
-  int chunks = (int)((npix + 255) / 256);
-  const int max_chunks = (132 * 8 + kblocks * cblocks - 1) / (kblocks * cblocks);
-  if (chunks > max_chunks) chunks = max_chunks;
-  if (chunks < 1) chunks = 1;
-  const int pix_per_cta = (int)((npix + chunks - 1) / chunks);
-  dim3 grid(kblocks * cblocks, chunks);
-  if (dtype == SPC_BF16)
-    wgrad_halo_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(p, kblocks, (int)npix, pix_per_cta, top, bot0, left, right0);
-  else
-    wgrad_halo_kernel<float><<<grid, 256, 0, st>>>(p, kblocks, (int)npix, pix_per_cta, top, bot0, left, right0);
-  spc::count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  return SPC_OK;
-}
-
 int launch_wgrad_direct(const DirectWgradParams& p_in, int dtype, cudaStream_t st) {
   DirectWgradParams p = p_in;
   if (p.rH == 0 && p.rW == 0) { p.ry0 = 0; p.rx0 = 0; p.rH = p.Ho; p.rW = p.Wo; }

@@ -17,8 +17,6 @@
 //
 // Warp roles (640 threads): 0 = TMA producer (activation row blocks and weight blocks, interleaved), 4..11 = two
 // consumer warpgroups, 12..19 = shifter.  All hand-offs are mbarriers; persistent CTAs, one per SM.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -53,8 +51,6 @@ struct TapParams {
   int opblk;                 // bytes of one 64-pixel block of an operand tile: cbox * 128
   int group;                 // 1: an operand-ring slot holds the S tiles of one filter ROW (one hand-shake per row), 0: one tap
   int rows_raw;              // NB + R - 1
-  int dbg;                   // SPC_TAP_DBG bit mask (timing experiments only, results are garbage): 1 no weight loads,
-                             // 2 no activation loads, 4 no output stores, 8 shifter does no data movement
   const __nv_bfloat16* bias;
   __nv_bfloat16* y;
 };
@@ -202,8 +198,7 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
       RingState rb, ra;
       const int xoff = SHIFT ? 8 : 0;
       int ct = blockIdx.x, ckc = 0;                       // current chunk (tile, channel chunk)
-      const bool noa = p.dbg & 1, noraw = p.dbg & 2;
-      if (ct < p.num_tiles && !noraw) {                   // its row blocks: all at once (nothing to overlap with yet)
+      if (ct < p.num_tiles) {                             // its row blocks: all at once (nothing to overlap with yet)
         TAP_TILE_DECODE(ct)
         mbar_wait(&raw_empty[rb.s], rb.ph ^ 1);
         mbar_arrive_expect_tx(&raw_full[rb.s], p.rows_raw * RAW_BLK);
@@ -214,13 +209,13 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
       while (ct < p.num_tiles) {
         int nt = ct, nkc = ckc + 1;                       // next chunk
         if (nkc == p.kchunks) { nkc = 0; nt = ct + gridDim.x; }
-        const bool has_next = nt < p.num_tiles && !noraw;
+        const bool has_next = nt < p.num_tiles;
         TAP_TILE_DECODE(has_next ? nt : ct)
         uint8_t* dst = raw_base + rb.s * p.rows_raw * RAW_BLK;
         bool armed = false;
         int row = 0;
         for (int tap = 0; tap < taps; ++tap) {
-          if (!p.a_resident && !noa) {
+          if (!p.a_resident) {
             mbar_wait(&a_empty[ra.s], ra.ph ^ 1);
             mbar_arrive_expect_tx(&a_full[ra.s], p.mrows * 128);
             tma_load_2d(a_base + ra.s * p.a_blk, &tmap_w, &a_full[ra.s], ckc * 64, tap * p.Mpad);
@@ -257,13 +252,13 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
       RingState rb, ro;
       for (int t = blockIdx.x; t < p.num_tiles; t += gridDim.x) {
         for (int kc = 0; kc < p.kchunks; ++kc) {
-          if (!(p.dbg & 2)) mbar_wait(&raw_full[rb.s], rb.ph);
+          mbar_wait(&raw_full[rb.s], rb.ph);
           // every channel row the MMA reads (KS * 16 = cbox): rows past Cin are zero, TMA zero-fills them in the raw box
-          const int cv = (p.dbg & 8) ? 0 : p.cbox;
+          const int cv = p.cbox;
           const uint8_t* rawb = raw_base + rb.s * p.rows_raw * RAW_BLK;
           for (int r = 0; r < p.R; ++r)
             ShiftRow<NB, S, 0>::run(rawb + r * RAW_BLK, RAW_BLK, cv, tid, op_base, p.opblk, p.group, op_full, op_empty, ro, p.ops);
-          if (!(p.dbg & 2)) mbar_arrive(&raw_empty[rb.s]);      // all shifter threads are done reading this raw buffer
+          mbar_arrive(&raw_empty[rb.s]);      // all shifter threads are done reading this raw buffer
           rb.next(p.rawb);
         }
       }
@@ -283,7 +278,7 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
       // previous one has completed (wgmma_wait<1>)
       int rel_op = -1, rel_a = -1, rel_raw = -1;
       for (int kc = 0; kc < p.kchunks; ++kc) {
-        if (!SHIFT && !(p.dbg & 2)) mbar_wait(&raw_full[rb.s], rb.ph);
+        if (!SHIFT) mbar_wait(&raw_full[rb.s], rb.ph);
         for (int tap = 0; tap < taps; ++tap) {
           uint32_t sb;
           const int si = tap % S;                                   // filter column (compile-time S)
@@ -297,7 +292,7 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
           if (p.a_resident) {
             sa = smem_u32(a_base + (tap * p.kchunks + kc) * p.a_blk);
           } else {
-            if (!(p.dbg & 1)) mbar_wait(&a_full[ra.s], ra.ph);
+            mbar_wait(&a_full[ra.s], ra.ph);
             sa = smem_u32(a_base + ra.s * p.a_blk);
           }
           wgmma_fence();
@@ -313,8 +308,8 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
           wgmma_wait<1>();
           if (wg_lead) {
             if (rel_op >= 0) mbar_arrive(&op_empty[rel_op]);
-            if (rel_a >= 0 && !(p.dbg & 1)) mbar_arrive(&a_empty[rel_a]);
-            if (rel_raw >= 0 && !(p.dbg & 2)) mbar_arrive(&raw_empty[rel_raw]);
+            if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);
+            if (rel_raw >= 0) mbar_arrive(&raw_empty[rel_raw]);
           }
           rel_op = rel_a = rel_raw = -1;
           if (SHIFT && (!p.group || si == S - 1)) { rel_op = ro.s; ro.next(p.ops); }
@@ -326,8 +321,8 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
       reg_fence(acc);
       if (wg_lead) {
         if (rel_op >= 0) mbar_arrive(&op_empty[rel_op]);
-        if (rel_a >= 0 && !(p.dbg & 1)) mbar_arrive(&a_empty[rel_a]);
-        if (rel_raw >= 0 && !(p.dbg & 2)) mbar_arrive(&raw_empty[rel_raw]);
+        if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);
+        if (rel_raw >= 0) mbar_arrive(&raw_empty[rel_raw]);
       }
       const int r0 = 64 * wg + 16 * w4 + (lane >> 2);   // fragment rows (output channels) r0 and r0 + 8
       const float b0 = (r0 < p.M && p.bias) ? __bfloat162float(p.bias[r0]) : 0.f;
@@ -352,7 +347,7 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
         fence_proxy_async();                              // smem writes -> visible to the TMA (async proxy)
         named_bar_sync(1, 256);
         // rows past the image and channels past M are clipped by the tensor map
-        if (leader && !(p.dbg & 4) && h0 + j < p.H) {
+        if (leader && h0 + j < p.H) {
           tma_store_4d(&tmap_y, stage_base, w0, h0 + j, 0, n_);
           tma_store_commit();
         }
@@ -455,10 +450,6 @@ int run_conv_tap_v2(const __nv_bfloat16* wp, int Mpad, int Cpad, const __nv_bflo
   SPC_REQUIRE(plan_tap(M, Cin, R, S, H, W, N, &pl), "tap conv: no shared-memory plan for M=%d Cin=%d %dx%d", M, Cin, R, S);
   TapParams& p = pl.p;
   p.ph = ph; p.Mpad = Mpad; p.bias = bias; p.y = y;
-  {
-    const char* e = getenv("SPC_TAP_DBG");   // read every call: dev probes flip it inside one process
-    p.dbg = e ? atoi(e) : 0;
-  }
   p.tiles_w = W / 64;
   p.tiles_h = (H + pl.NB - 1) / pl.NB;
   p.num_tiles = p.tiles_w * p.tiles_h * N;

@@ -25,7 +25,7 @@ static long long g_launches = 0;
 void count_launch(int n) { g_launches += n; }
 long long launches(int reset) { long long v = g_launches; if (reset) g_launches = 0; return v; }
 
-// grow-only device scratch for the boundary patches (single host thread per process)
+// grow-only device scratch for the halo fix-up (single host thread per process)
 static void* g_scratch = nullptr;
 static size_t g_scratch_bytes = 0;
 void* boundary_scratch(size_t bytes) {
@@ -118,47 +118,6 @@ __global__ void mailbox_wait_kernel(const uint32_t* flag, uint32_t seq, unsigned
       }
     }
   } while (true);
-}
-
-// ---- boundary patches -------------------------------------------------------------------------
-// gather:  P[n][c][r][q] = view(n, c, h0 + r, w0 + q)   (tile + halo strips, zero elsewhere)
-// gather_dy: G[n][k][r][q] = dy[n][k][y0 + r - ph][x0 + q - pw] inside the output rect, else 0
-// scatter: y[n][k][y0 + i][x0 + j] = O[n][k][ph + i][pw + j]
-template <typename T>
-__global__ void patch_gather_kernel(const TileView v, T* __restrict__ P, int Hp, int Wp, int h0, int w0) {
-  const size_t total = (size_t)v.N * v.C * Hp * Wp;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int q = (int)(i % Wp);
-    const int r = (int)((i / Wp) % Hp);
-    const size_t nc = i / ((size_t)Wp * Hp);
-    const T* ptr = tile_ptr<T>(v, (int)(nc / v.C), (int)(nc % v.C), h0 + r, w0 + q);
-    P[i] = ptr ? __ldg(ptr) : from_f32<T>(0.f);
-  }
-}
-template <typename T>
-__global__ void patch_gather_dy_kernel(const T* __restrict__ dy, T* __restrict__ G, int NK, int Ho, int Wo, int Hp,
-                                       int Wp, int y0, int x0, int rh, int rw, int ph, int pw) {
-  const size_t total = (size_t)NK * Hp * Wp;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int q = (int)(i % Wp);
-    const int r = (int)((i / Wp) % Hp);
-    const size_t nk = i / ((size_t)Wp * Hp);
-    const int ii = r - ph, jj = q - pw;
-    T val = from_f32<T>(0.f);
-    if ((unsigned)ii < (unsigned)rh && (unsigned)jj < (unsigned)rw) val = dy[(nk * Ho + y0 + ii) * Wo + x0 + jj];
-    G[i] = val;
-  }
-}
-template <typename T>
-__global__ void patch_scatter_kernel(const T* __restrict__ O, T* __restrict__ y, int NK, int Ho, int Wo, int Hp, int Wp,
-                                     int y0, int x0, int rh, int rw, int ph, int pw) {
-  const size_t total = (size_t)NK * rh * rw;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int j = (int)(i % rw);
-    const int ii = (int)((i / rw) % rh);
-    const size_t nk = i / ((size_t)rw * rh);
-    y[(nk * Ho + y0 + ii) * Wo + x0 + j] = O[(nk * Hp + ph + ii) * Wp + pw + j];
-  }
 }
 
 // ---- fused protocol kernels -----------------------------------------------------------------
@@ -394,39 +353,6 @@ int launch_boundary_scatter(const void* O, const BoundaryRects& b, int K, int Ho
   const size_t total = (size_t)K * b.total;
   if (!total) return SPC_OK;
   boundary_scatter_kernel<<<grid_for(total), 256, 0, st>>>((const __nv_bfloat16*)O, b, K, Ho, Wo, (__nv_bfloat16*)y);
-  count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  return SPC_OK;
-}
-int launch_patch_gather(const TileView& v, void* P, int Hp, int Wp, int h0, int w0, int dtype, cudaStream_t st) {
-  const size_t total = (size_t)v.N * v.C * Hp * Wp;
-  if (!total) return SPC_OK;
-  if (dtype == SPC_BF16) patch_gather_kernel<__nv_bfloat16><<<grid_for(total), 256, 0, st>>>(v, (__nv_bfloat16*)P, Hp, Wp, h0, w0);
-  else patch_gather_kernel<float><<<grid_for(total), 256, 0, st>>>(v, (float*)P, Hp, Wp, h0, w0);
-  count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  return SPC_OK;
-}
-int launch_patch_gather_dy(const void* dy, void* G, int NK, int Ho, int Wo, int Hp, int Wp, int y0, int x0, int rh, int rw,
-                           int ph, int pw, int dtype, cudaStream_t st) {
-  const size_t total = (size_t)NK * Hp * Wp;
-  if (!total) return SPC_OK;
-  if (dtype == SPC_BF16)
-    patch_gather_dy_kernel<__nv_bfloat16><<<grid_for(total), 256, 0, st>>>((const __nv_bfloat16*)dy, (__nv_bfloat16*)G, NK, Ho, Wo, Hp, Wp, y0, x0, rh, rw, ph, pw);
-  else
-    patch_gather_dy_kernel<float><<<grid_for(total), 256, 0, st>>>((const float*)dy, (float*)G, NK, Ho, Wo, Hp, Wp, y0, x0, rh, rw, ph, pw);
-  count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  return SPC_OK;
-}
-int launch_patch_scatter(const void* O, void* y, int NK, int Ho, int Wo, int Hp, int Wp, int y0, int x0, int rh, int rw,
-                         int ph, int pw, int dtype, cudaStream_t st) {
-  const size_t total = (size_t)NK * rh * rw;
-  if (!total) return SPC_OK;
-  if (dtype == SPC_BF16)
-    patch_scatter_kernel<__nv_bfloat16><<<grid_for(total), 256, 0, st>>>((const __nv_bfloat16*)O, (__nv_bfloat16*)y, NK, Ho, Wo, Hp, Wp, y0, x0, rh, rw, ph, pw);
-  else
-    patch_scatter_kernel<float><<<grid_for(total), 256, 0, st>>>((const float*)O, (float*)y, NK, Ho, Wo, Hp, Wp, y0, x0, rh, rw, ph, pw);
   count_launch();
   SPC_CHECK_CUDA(cudaGetLastError());
   return SPC_OK;

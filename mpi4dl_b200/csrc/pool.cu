@@ -4,8 +4,6 @@
 // exchange + 8 unpack copies) followed by nn.{Max,Avg}Pool2d(padding=0).  Here the window is
 // read straight from the tile and its halo strips (TileView); the padded tensor never exists.
 // These ops are pure HBM streaming (AI ~ 0): one read of x, one write of y.
-#include <stdlib.h>
-
 #include <cuda.h>
 
 #include "common.cuh"
@@ -210,146 +208,9 @@ pool3_fwd_kernel(const PoolParams p) {
   }
 }
 
-// ---- forward, 3x3 stride 1, one output vector per thread, all nine loads independent ---------
-// Rows h-1, h, h+1: one 16-byte vector each plus the two overhang elements as plain scalar loads
-// (L1 hits: the neighbouring lanes fetch the same lines).  No shuffles, no divergence away from
-// the tile edge, high memory-level parallelism; row re-reads are served by L1/L2.
-template <typename T, int VEC>
-__global__ void __launch_bounds__(256)
-pool3_s1_simple_kernel(const PoolParams p) {
-  const int W = p.in.W, H = p.in.H;
-  const int wv = W / VEC;
-  const size_t total = (size_t)p.in.N * p.in.C * H * wv;
-  const float inv = 1.f / 9.f;
-  const bool is_max = p.mode == SPC_POOL_MAX;
-  const T* x = reinterpret_cast<const T*>(p.in.x);
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int vx = (int)(i % wv);
-    const size_t rowid = i / wv;              // nc * H + oy
-    const int oy = (int)(rowid % H);
-    const size_t nc = rowid / H;
-    const int w0 = vx * VEC;
-    const bool interior = (oy > 0) && (oy < H - 1) && (vx > 0) && (vx < wv - 1);
-    float acc[VEC];
-#pragma unroll
-    for (int q = 0; q < VEC; ++q) acc[q] = is_max ? -INFINITY : 0.f;
-    if (interior) {
-      const T* r0 = x + (rowid - 1) * W + w0;
-      float b[3][VEC], l[3], r[3];
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-        load_vec<T, VEC>(r0 + (size_t)a * W, b[a]);
-        l[a] = to_f32<T>(__ldg(r0 + (size_t)a * W - 1));
-        r[a] = to_f32<T>(__ldg(r0 + (size_t)a * W + VEC));
-      }
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int q = 0; q < VEC; ++q) {
-          const float lo = q == 0 ? l[a] : b[a][q - 1];
-          const float hi = q == VEC - 1 ? r[a] : b[a][q + 1];
-          acc[q] = is_max ? fmaxf(acc[q], fmaxf(fmaxf(lo, b[a][q]), hi)) : acc[q] + (lo + b[a][q] + hi);
-        }
-    } else {
-      const int c = (int)(nc % p.in.C), n = (int)(nc / p.in.C);
-      for (int a = -1; a <= 1; ++a)
-#pragma unroll
-        for (int q = 0; q < VEC; ++q)
-          for (int bb = -1; bb <= 1; ++bb) {
-            const float v = tile_load<T>(p.in, n, c, oy + a, w0 + q + bb);
-            acc[q] = is_max ? fmaxf(acc[q], v) : acc[q] + v;
-          }
-    }
-    float outv[VEC];
-#pragma unroll
-    for (int q = 0; q < VEC; ++q) outv[q] = is_max ? acc[q] : acc[q] * inv;
-    store_vec<T, VEC>(reinterpret_cast<T*>(p.out) + rowid * W + w0, outv);
-  }
-}
-
-// ---- forward, 3x3 stride 1, rolling window ---------------------------------------------------
-// Each thread owns a strip of VEC columns and walks RB consecutive output rows, loading every
-// input row ONCE (16-byte vector + two warp shuffles for the overhang) and keeping the last
-// three horizontal partial results in registers: input is read (RB+2)/RB times instead of 3x.
-template <typename T, int VEC, int RB>
-__global__ void __launch_bounds__(256, 3)
-pool3_s1_rolling_kernel(const PoolParams p) {
-  static_assert(VEC * sizeof(T) == 16, "one 16-byte vector per thread per row");
-  constexpr int PF = 4;                      // rows prefetched ahead (memory-level parallelism)
-  const int wv = p.in.W / VEC;               // multiple of 32: a warp never straddles two strips
-  const int rblocks = (p.in.H + RB - 1) / RB;
-  const size_t total = (size_t)p.in.N * p.in.C * rblocks * wv;
-  const float inv = 1.f / 9.f;
-  const bool is_max = p.mode == SPC_POOL_MAX;
-  const T* x = reinterpret_cast<const T*>(p.in.x);
-  const int lane = threadIdx.x & 31;
-  const size_t warp0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) - lane;
-  for (size_t base = warp0; base < total; base += (size_t)gridDim.x * blockDim.x) {
-    const size_t i = base + lane;            // total % 32 == 0: every lane is valid
-    const int vx = (int)(i % wv);
-    const int rb = (int)((i / wv) % rblocks);
-    const size_t nc = i / ((size_t)wv * rblocks);
-    const int c = (int)(nc % p.in.C), n = (int)(nc / p.in.C);
-    const int w0 = vx * VEC;
-    const int h_begin = rb * RB, h_end = min(p.in.H, h_begin + RB);   // rows h_begin-1 .. h_end are read
-    const T* plane = x + nc * (size_t)p.in.H * p.in.W + w0;
-    uint4 pf[PF];
-#pragma unroll
-    for (int k = 0; k < PF; ++k) {
-      const int hc = min(max(h_begin - 1 + k, 0), p.in.H - 1);
-      pf[k] = __ldg(reinterpret_cast<const uint4*>(plane + (size_t)hc * p.in.W));
-    }
-    float h0v[VEC], h1v[VEC], h2v[VEC];      // horizontal 3-reductions of rows h-2, h-1, h
-#pragma unroll
-    for (int q = 0; q < VEC; ++q) { h0v[q] = 0.f; h1v[q] = 0.f; h2v[q] = 0.f; }
-#pragma unroll 1
-    for (int hb = h_begin - 1; hb <= h_end; hb += PF) {
-#pragma unroll
-      for (int k = 0; k < PF; ++k) {
-        const int h = hb + k;
-        if (h <= h_end) {                    // warp-uniform
-          const uint4 cur = pf[k];
-          if (h + PF <= h_end) {
-            const int hc = min(h + PF, p.in.H - 1);
-            pf[k] = __ldg(reinterpret_cast<const uint4*>(plane + (size_t)hc * p.in.W));
-          }
-          float body[VEC];
-          const T* e = reinterpret_cast<const T*>(&cur);
-          const bool row_in = (unsigned)h < (unsigned)p.in.H;
-#pragma unroll
-          for (int q = 0; q < VEC; ++q) body[q] = row_in ? to_f32<T>(e[q]) : tile_load<T>(p.in, n, c, h, w0 + q);
-          float left = __shfl_up_sync(0xffffffffu, body[VEC - 1], 1);
-          float right = __shfl_down_sync(0xffffffffu, body[0], 1);
-          // warp-boundary lanes: a plain scalar load when the neighbour column is inside the tile
-          // (the common case); the halo / zero-padding lookup only at the tile's own edge
-          if (vx == 0) left = tile_load<T>(p.in, n, c, h, w0 - 1);
-          else if (lane == 0) left = row_in ? to_f32<T>(plane[(size_t)h * p.in.W - 1]) : tile_load<T>(p.in, n, c, h, w0 - 1);
-          if (vx == wv - 1) right = tile_load<T>(p.in, n, c, h, w0 + VEC);
-          else if (lane == 31) right = row_in ? to_f32<T>(plane[(size_t)h * p.in.W + VEC]) : tile_load<T>(p.in, n, c, h, w0 + VEC);
-#pragma unroll
-          for (int q = 0; q < VEC; ++q) {
-            h0v[q] = h1v[q];
-            h1v[q] = h2v[q];
-            const float a = q == 0 ? left : body[q - 1];
-            const float b = q == VEC - 1 ? right : body[q + 1];
-            h2v[q] = is_max ? fmaxf(fmaxf(a, body[q]), b) : (a + body[q] + b);
-          }
-          if (h >= h_begin + 1) {            // rows h-2, h-1, h form the window of output row h-1
-            float outv[VEC];
-#pragma unroll
-            for (int q = 0; q < VEC; ++q)
-              outv[q] = is_max ? fmaxf(fmaxf(h0v[q], h1v[q]), h2v[q]) : (h0v[q] + h1v[q] + h2v[q]) * inv;
-            store_vec<T, VEC>(reinterpret_cast<T*>(p.out) + ((nc * p.Ho) + (h - 1)) * (size_t)p.Wo + w0, outv);
-          }
-        }
-      }
-    }
-  }
-}
-
 // ---- forward, 3x3 stride 1, TMA-staged ----------------------------------------------------------
-// The rolling kernel above is latency/occupancy bound (1.8 TB/s): each warp keeps only a few
-// 16-byte loads in flight.  Here one producer thread per CTA keeps P3_STAGES bulk-tensor loads of
+// A kernel whose warps load their own 16-byte vectors keeps only a few loads in flight per warp and
+// is latency/occupancy bound.  Here one producer thread per CTA keeps P3_STAGES bulk-tensor loads of
 // whole (64+2) x (16*VEC + 2*VEC) input boxes in flight; TMA's out-of-bounds zero fill IS the zero
 // padding, so the 256 consumer threads run a branch-free stencil out of shared memory (one 16-byte
 // vector per thread per row, neighbours by shuffle) and store 16 bytes per thread per output row.
@@ -484,10 +345,12 @@ typedef CUresult (*P3EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, vo
                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// x viewed as [planes][H][W]; returns SPC_OK and launches, or a negative value when TMA cannot be used
+// x viewed as [planes][H][W]
 template <typename T>
 int launch_pool3_tma(const PoolParams& p, cudaStream_t st) {
   using G = P3Geom<T>;
+  SPC_REQUIRE(p.in.x != nullptr && (uintptr_t)p.in.x % 16 == 0 && ((size_t)p.in.W * sizeof(T)) % 16 == 0,
+              "pool: TMA needs a 16-byte aligned input and row pitch (W=%d)", p.in.W);
   static P3EncodeFn enc = nullptr;
   if (!enc) {
     void* fp = nullptr;
@@ -549,13 +412,6 @@ int launch_pool3_tma(const PoolParams& p, cudaStream_t st) {
     SPC_CHECK_CUDA(cudaGetLastError());
   }
   return SPC_OK;
-}
-
-// TMA needs: 16-byte aligned base and row pitch, planes*H*W addressable by the 3-D map
-template <typename T>
-bool pool3_tma_ok(const PoolParams& p) {
-  return getenv("SPC_POOL_NOTMA") == nullptr && p.in.x != nullptr && (uintptr_t)p.in.x % 16 == 0 &&
-         ((size_t)p.in.W * sizeof(T)) % 16 == 0 && p.in.H >= 1 && p.in.W >= 1;
 }
 
 // ---- backward: one thread per dx element (gather over the windows that cover it) -------------
@@ -689,17 +545,8 @@ int run_fwd(const PoolParams& p, cudaStream_t st) {
                       p.in.W == p.Wo * p.stride;
   const size_t vtotal = total / VEC;
   const int blocks = (int)((vtotal + 255) / 256 > 132 * 32 ? 132 * 32 : (vtotal + 255) / 256);
-  if (vec_ok && p.k == 3 && p.stride == 1 && pool3_tma_ok<T>(p)) {
+  if (vec_ok && p.k == 3 && p.stride == 1) {
     return launch_pool3_tma<T>(p, st);
-  } else if (vec_ok && p.k == 3 && p.stride == 1 && p.in.W % (VEC * 32) != 0) {
-    pool3_fwd_kernel<T, VEC, 1><<<blocks, 256, 0, st>>>(p);
-  } else if (vec_ok && p.k == 3 && p.stride == 1 && getenv("SPC_POOL_SIMPLE") != nullptr) {
-    pool3_s1_simple_kernel<T, VEC><<<blocks, 256, 0, st>>>(p);
-  } else if (vec_ok && p.k == 3 && p.stride == 1) {
-    constexpr int RB = 16;
-    const size_t items = (size_t)p.in.N * p.in.C * ((p.in.H + RB - 1) / RB) * (p.in.W / VEC);
-    const int b3 = (int)((items + 255) / 256 > 132 * 16 ? 132 * 16 : (items + 255) / 256);
-    pool3_s1_rolling_kernel<T, VEC, RB><<<b3, 256, 0, st>>>(p);
   } else if (vec_ok && p.k == 3 && p.stride == 2) {
     pool3_fwd_kernel<T, VEC, 2><<<blocks, 256, 0, st>>>(p);
   } else if (vec_ok && p.k == 2 && p.stride == 2) {
@@ -725,16 +572,7 @@ int run_bwd(const PoolParams& p, cudaStream_t st) {
     PoolParams q = p;
     q.in = make_view(p.dy, nullptr, p.in.N, p.in.C, p.Ho, p.Wo, 1, 1);
     q.dy = nullptr;
-    constexpr int VEC = 16 / sizeof(T);
-    const size_t vt = total / VEC;
-    constexpr int RB = 16;
-    const size_t items = (size_t)q.in.N * q.in.C * ((q.in.H + RB - 1) / RB) * (q.in.W / VEC);
-    const int b2 = (int)((items + 255) / 256 > 132 * 16 ? 132 * 16 : (items + 255) / 256);
-    const int b1 = (int)((vt + 255) / 256 > 132 * 32 ? 132 * 32 : (vt + 255) / 256);
-    if (pool3_tma_ok<T>(q)) return launch_pool3_tma<T>(q, st);
-    if (getenv("SPC_POOL_SIMPLE") != nullptr) pool3_s1_simple_kernel<T, VEC><<<b1, 256, 0, st>>>(q);
-    else if (q.in.W % (VEC * 32) == 0) pool3_s1_rolling_kernel<T, VEC, RB><<<b2, 256, 0, st>>>(q);
-    else pool3_fwd_kernel<T, VEC, 1><<<b1, 256, 0, st>>>(q);
+    return launch_pool3_tma<T>(q, st);
   } else if (even && p.mode == SPC_POOL_AVG && p.k == 3 && p.stride == 2) {
     const size_t vt = total / 32;
     const int b2 = (int)((vt + 255) / 256 > 132 * 32 ? 132 * 32 : (vt + 255) / 256);

@@ -220,7 +220,8 @@ def test_conv_against_oracle_seeded(case, dtype):
 
 POOL_CASES = [("avg", 3, 1, 16, 64), ("avg", 3, 2, 32, 64), ("max", 2, 2, 16, 32), ("max", 3, 1, 9, 11),
               ("avg", 3, 1, 7, 13), ("avg", 3, 2, 10, 18), ("max", 3, 2, 8, 8), ("avg", 5, 1, 12, 12),
-              ("avg", 3, 1, 20, 256), ("max", 3, 1, 33, 512), ("avg", 3, 2, 34, 256),   # rolling-window kernel
+              # rows of whole warps of 16-byte vectors (forward: 3x3 s1 on the TMA kernel, 3x3 s2 on pool3_fwd_kernel)
+              ("avg", 3, 1, 20, 256), ("max", 3, 1, 33, 512), ("avg", 3, 2, 34, 256),
               # TMA-staged 3x3 s1 kernel: several row / column tiles, partial edge tiles, tiny planes
               ("avg", 3, 1, 70, 136), ("max", 3, 1, 130, 264), ("avg", 3, 1, 64, 128), ("avg", 3, 1, 2, 16),
               ("max", 3, 1, 1, 8)]

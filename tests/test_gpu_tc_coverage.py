@@ -16,7 +16,7 @@ element (the inputs are bf16-representable, so only the fp32 summation and the f
     dw, db (fp32)      |got - ref| <= 2^-12 A           (straight from spc_conv2d_wgrad, not rounded by autograd)
 tests/test_tc_coverage_bounds.py checks on the CPU that these bounds reject a dropped channel, a dropped pixel row
 and a dropped tap at the table's shapes, and tests/test_tc_coverage_bounds.py::test_instance_table_matches_library
-that the table (plus UNREACHABLE) names exactly the instances libspconv.so contains.  Run with -s to see the worst
+that the table names exactly the instances libspconv.so contains.  Run with -s to see the worst
 err / bound of every case and, at the end, per kernel family.
 """
 import collections
@@ -163,26 +163,16 @@ CASES = [
          "generic subsampled copies; dgrad on the direct kernel"),
 ]
 
-# what the halo fix-up launches (test_halo_masks): the im2col + pointwise-GEMM fix-up, and with SPC_BOUNDARY_V1=1 the
-# per-rectangle patches (stride 1)
+# what the bf16 halo fix-up launches (test_halo_masks): im2col of the boundary outputs + one pointwise GEMM
 FIXUP_FWD = K("halo_im2col_kernel", "boundary_scatter_kernel")
 FIXUP_WGRAD = K("halo_im2col_kernel", "boundary_gather_kernel")
-PATCH_FWD = K("patch_gather_kernel<__nv_bfloat16>", "patch_scatter_kernel<__nv_bfloat16>")
-PATCH_WGRAD = K("patch_gather_kernel<__nv_bfloat16>", "patch_gather_dy_kernel<__nv_bfloat16>")
-
-# instances compiled into the library that no descriptor can reach
-UNREACHABLE = {
-    parse_kernel("patch_gather_kernel<float>"): "the patch path requires bf16 (patch_ok): fp32 runs the direct kernel",
-    parse_kernel("patch_gather_dy_kernel<float>"): "the patch path requires bf16 (patch_ok)",
-    parse_kernel("patch_scatter_kernel<float>"): "the patch path requires bf16 (patch_ok)",
-}
 
 
 def table_instances():
     out = set()
     for c in CASES:
         out |= c.launches
-    return out | FIXUP_FWD | FIXUP_WGRAD | PATCH_FWD | PATCH_WGRAD
+    return out | FIXUP_FWD | FIXUP_WGRAD
 
 
 def case_id(c):
@@ -293,9 +283,9 @@ def _st():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def desc(c, N=None):
+def desc(c, N=None, dtype=_lib.SPC_BF16, algo=_lib.SPC_ALGO_AUTO):
     return _lib.ConvDesc(c.N if N is None else N, c.C, c.H, c.W, c.K, c.R, c.S, c.stride, c.stride, (c.R - 1) // 2,
-                         (c.S - 1) // 2, _lib.SPC_BF16, _lib.SPC_ALGO_AUTO)
+                         (c.S - 1) // 2, dtype, algo)
 
 
 def _ws(d, op):
@@ -354,7 +344,7 @@ def traced(fn):
 
 
 FAMILIES = ("conv_tap_kernel", "wgrad_tap_kernel", "pw_gemm_kernel", "pw_wgrad_kernel", "conv_direct_kernel",
-            "wgrad_halo_kernel", "wgrad_direct_kernel")
+            "wgrad_direct_kernel")
 WORST = collections.defaultdict(float)
 
 
@@ -462,31 +452,53 @@ def _masks(c, method, P):
     return out
 
 
-@pytest.mark.parametrize("v1", [0, 1], ids=["fixup", "boundary_v1"])
+# the fix-up paths of test_halo_masks: "fixup" is bf16 on the boundary GEMM (fprop and wgrad); the direct ones are
+# spc_conv2d_fwd_interior + spc_conv2d_fwd_boundary with the direct kernel on the boundary rectangles, which fp32 and
+# SPC_ALGO_DIRECT use (the overlapped forward of conv_spatial in fp32)
+DIRECT_PATHS = {"direct_fp32": (torch.float32, _lib.SPC_F32, _lib.SPC_ALGO_AUTO),
+                "direct_bf16": (torch.bfloat16, _lib.SPC_BF16, _lib.SPC_ALGO_DIRECT)}
+
+
+def run_boundary_direct(c, mask, tag, dtype, spc_dtype, algo):
+    """interior pass, then the boundary pass; y against the fp64 reference.  Returns the kernels the boundary pass
+    launched and a function that traces it again"""
+    L = _lib.lib()
+    x, w, b, dy, strips = make_inputs(c, mask)
+    ref, A = reference(x, w, b, dy, strips, c.stride)
+    x, w, b, *strips = [t.to(DEV, dtype) if t is not None else None for t in (x, w, b, *strips)]
+    d = desc(c, dtype=spc_dtype, algo=algo)
+    assert not L.spc_conv_uses_tcgen05(C.byref(d), 0), tag
+    y = torch.empty((c.N, c.K) + out_hw(c), dtype=dtype, device=DEV)
+    _lib.check(L.spc_conv2d_fwd_interior(C.byref(d), _ptr(x), _ptr(w), _ptr(b), _ptr(y), None, 0, _st()), "fwd_interior")
+    halo = _lib.make_halo(strips)
+
+    def boundary():
+        _lib.check(L.spc_conv2d_fwd_boundary(C.byref(d), _ptr(x), C.byref(halo), _ptr(w), _ptr(b), _ptr(y), _st()),
+                   "fwd_boundary")
+
+    _, k = traced(boundary)
+    _record(tag, "y", k, check_act(y, ref["y"], A["y"], tag + " y"))
+    return k, lambda: traced(boundary)[1]
+
+
+@pytest.mark.parametrize("path", ["fixup"] + list(DIRECT_PATHS))
 @pytest.mark.parametrize("grid", GRIDS, ids=[g[0] for g in GRIDS])
 @pytest.mark.parametrize("c", MASK_CASES, ids=case_id)
-def test_halo_masks(c, grid, v1, monkeypatch):
+def test_halo_masks(c, grid, path):
     """corner, edge and interior tiles of a 3x3 grid and the end / middle tiles of 3-way slicing: the bf16 halo
-    fix-up (SPC_BOUNDARY_V1=1: per-rectangle patches for stride 1, direct-kernel strips for stride 2)"""
-    if v1:
-        monkeypatch.setenv("SPC_BOUNDARY_V1", "1")
-    else:
-        monkeypatch.delenv("SPC_BOUNDARY_V1", raising=False)
+    fix-up on the boundary GEMM, and the forward fix-up on the direct kernel (fp32, bf16 with SPC_ALGO_DIRECT)"""
     method, P = grid
     for mask in _masks(c, method, P):
-        tag = "%s %s%s %s" % (case_id(c), method, "".join(map(str, mask)), "v1" if v1 else "")
-        kf, kd, kw, rest = run_and_check(c, mask, tag, split_check=True)
-        k, retrace = kf | kd | kw, rest[-1]
+        tag = "%s %s%s %s" % (case_id(c), method, "".join(map(str, mask)), path)
         fix = _fixup_expected(c, mask)
-        if not v1:
-            assert launched(k, lambda k: FIXUP_FWD | FIXUP_WGRAD <= k, retrace) == fix, (tag, fix, sorted(k))
-        elif c.stride == 1:
-            assert launched(k, lambda k: PATCH_FWD | PATCH_WGRAD <= k, retrace) == fix, (tag, fix, sorted(k))
-            assert not (FIXUP_FWD | FIXUP_WGRAD) & k, tag
-        else:   # strided layers: the direct kernel on the boundary strips, and over the strips for wgrad
+        if path == "fixup":
+            kf, kd, kw, rest = run_and_check(c, mask, tag, split_check=True)
+            k = kf | kd | kw
+            assert launched(k, lambda k: FIXUP_FWD | FIXUP_WGRAD <= k, rest[-1]) == fix, (tag, fix, sorted(k))
+        else:
+            k, retrace = run_boundary_direct(c, mask, tag, *DIRECT_PATHS[path])
             assert launched(k, lambda k: "conv_direct_kernel" in _names(k), retrace) == fix, (tag, fix, sorted(k))
-            assert launched(k, lambda k: "wgrad_halo_kernel" in _names(k), retrace) == any(mask), (tag, sorted(k))
-            assert not (FIXUP_FWD | FIXUP_WGRAD) & k, tag
+            assert "halo_im2col_kernel" not in _names(k), (tag, sorted(k))
 
 
 TAP_CASES = [c for c in CASES if c.stride == 1 and c.R * c.S > 1]
