@@ -16,7 +16,8 @@
 //     wgmma and write each tile row through a swizzled staging block and a TMA store.
 //
 // Warp roles (640 threads): 0 = TMA producer (activation row blocks and weight blocks, interleaved), 4..11 = two
-// consumer warpgroups, 12..19 = shifter.  All hand-offs are mbarriers; persistent CTAs, one per SM.
+// consumer warpgroups, 12..19 = shifter; setmaxnreg moves the registers of the producer warpgroup and the shifters to
+// the consumers.  All hand-offs are mbarriers; persistent CTAs, one per SM.
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -180,13 +181,17 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
   const int n_ = (t) / (p.tiles_w * p.tiles_h);                   \
   const int w0 = tw_ * 64, h0 = th_ * NB;
 
-  if (warp == 0) {
+  // 640 x 96 registers at launch.  The producer warpgroup (one busy thread) and the shifters (S = 1: idle) hand theirs
+  // to the consumers, whose accumulators would spill at 96: 24 + 2 x 80 + 2 x 144 (S = 1: 24 + 2 x 24 + 2 x 200) <= 480.
+  // Each role sets its count at the top of its own branch, so that ptxas allocates that branch at that count.
+  if (warp < 4) {
+    setmaxnreg_dec<24>();
     // ================= TMA producer: activation row blocks + (streamed) weight blocks =================
     // One thread issues both, INTERLEAVED: the TMA unit serves a CTA's requests in order, so a burst of all row
     // blocks of the next chunk (80 KB) in front of the small per-tap weight loads starved the MMA of weights for
     // ~2 us per chunk (r2 ncu: tensor pipe 24 %, L2->SM 4.4 TB/s).  Row blocks of chunk g+1 are therefore
     // spread over the taps of chunk g, behind each tap's weight block.
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       tma_prefetch_desc(&tmap_x);
       tma_prefetch_desc(&tmap_w);
       if (p.a_resident) {
@@ -246,6 +251,7 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
       }
     }
   } else if (warp >= 12) {
+    setmaxnreg_dec<SHIFT ? 80 : 24>();
     // ================= shifter: raw row blocks -> swizzled operand tile of tap (r, s) =================
     if (SHIFT) {
       const int tid = threadIdx.x - 12 * 32;   // 0..255
@@ -263,7 +269,8 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
         }
       }
     }
-  } else if (threadIdx.x >= 128) {
+  } else {
+    setmaxnreg_inc<SHIFT ? 144 : 200>();
     // ================= consumers: wgmma over (chunk, tap), then registers -> NCHW rows =================
     const int wg = (threadIdx.x >> 7) - 1;
     const int w4 = (threadIdx.x >> 5) & 3;

@@ -123,6 +123,16 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
+// warp-specialised register reallocation: every warp of a warpgroup executes the same setmaxnreg; the per-thread counts
+// of all warpgroups must fit the registers the CTA was launched with (threads x the kernel's register count)
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
 // keep the accumulator registers live across wgmma_wait (the compiler does not see the async writes)
 template <int R>
 __device__ __forceinline__ void reg_fence(float (&d)[R]) {

@@ -12,11 +12,15 @@
 // with both tap indices mirrored (dW[k][c][R-1-r][S-1-s]).
 // Line buffer: a CTA walks down a 64-pixel-wide column strip; step j = P row ha + j meets Q rows j .. j + R' - 1 of a
 // ring of shifted row tile-sets, so every Q row is loaded and shifted once and used by R' steps.  Accumulators of the
-// NT = 128 / QC taps of a pass live in the registers of two consumer warpgroups (64 fp32 per thread; more taps -> more
-// passes over the strip); fp32 atomics at the end.  Every k-step issues all NT wgmma (the last pass may have fewer
-// taps: its spare accumulators repeat the last tap and are not flushed), so none sits under a data-dependent branch.
+// NT = 256 / QC taps of a pass live in the registers of two consumer warpgroups (<= 128 fp32 per thread; more taps ->
+// more passes over the strip); fp32 atomics at the end.  A pass with fewer than NT taps skips the wgmma of its spare
+// accumulators (a warp-uniform branch; ptxas does not serialise the wgmma for it) and does not flush them.
+// All passes of a filter run in one launch: the pass is the fastest-varying part of the work item, so the passes of
+// one (image, strip, row range) run on neighbouring CTAs at the same time and read the same P and Q rows, which come
+// from HBM once and from L2 for the other passes.
 //
-// Warp roles (640 threads): 0 = TMA producer, 4..11 = two consumer warpgroups (wgmma + flush), 12..19 = shifter.
+// Warp roles (640 threads): 0 = TMA producer, 4..11 = two consumer warpgroups (wgmma + flush), 12..19 = shifter;
+// setmaxnreg moves the registers of the producer warpgroup and the shifters to the consumers.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -38,6 +42,7 @@ constexpr int RAW_ROW = 160;       // raw Q row: [Qch][80 px], dense rows of 160
 constexpr int MAXP = 8;            // P row stages (ring depths are chosen by the launcher: bytes in flight)
 constexpr int MAXRAW = 8;          // raw Q row slots
 constexpr int MAXQ = 16;           // Q row ring slots
+constexpr int MAXPASS = 8;         // tap rectangles of one filter (<= 7: R or S <= 7 and >= 2 taps per pass)
 
 struct WtParams {
   float* dw;
@@ -49,14 +54,16 @@ struct WtParams {
   int p_blk;                   // P stage stride (1024-aligned)
   int qt_bytes;                // one shifted Q tile: Qc16 * 128
   int ph, pw;
-  // this launch's tap rectangle (a "pass"): filter rows [r0, r0 + nr), columns [s0, s0 + ns)
-  int r0, nr, s0, ns;
-  int rq;                      // Q row ring slots (>= nr + 1)
+  // tap rectangles ("passes"): filter rows [r0, r0 + nr), columns [s0, s0 + ns) = rect[pass][0..3]
+  int npass;
+  int rect[MAXPASS][4];
+  int nr_max, ns_max;          // the largest pass rectangle: the shared-memory rings are sized for it
+  int rq;                      // Q row ring slots (>= nr_max + 1)
   int psn, rawn;               // P row stages, raw Q row slots
   int nbw;                     // 64-pixel blocks per strip row (strip width = 64 * nbw): rows of few channels are
                                // small, and the TMA loads are latency-bound -> wider strips keep more bytes in flight
   int raw_bytes;               // raw Q row bytes: Qc16 * 160
-  int strips, row_splits, rows_per_split, num_items;
+  int strips, row_splits, rows_per_split, num_items;   // num_items = N * strips * row_splits * npass
 };
 
 struct Ring {
@@ -82,34 +89,35 @@ __device__ __forceinline__ uint4 shift_window(const uint32_t (&w)[8]) {
   return o;
 }
 
-// write the shifted tiles of filter columns [s0, s0 + ns) of one raw Q row; tile of column s sits at (s - s0) * qt_bytes
+// write the shifted tiles of filter columns [s0, s0 + ns) of one raw Q row for channels cb and cb + 32; the tile of
+// column s sits at (s - s0) * qt_bytes
 template <int S, int SI>
 struct ShiftCols {
-  static __device__ __forceinline__ void run(const uint32_t (&win)[4][8], int qc16, int tid, uint8_t* dst, int qt_bytes, int s0,
-                                             int ns) {
+  static __device__ __forceinline__ void run(const uint32_t (&win)[2][8], int cb, int qc16, int q, uint8_t* dst, int qt_bytes,
+                                             int s0, int ns) {
     if constexpr (SI < S) {
       if (SI >= s0 && SI < s0 + ns) {
-        const int q = tid & 7, c0 = tid >> 3;
         uint8_t* t = dst + (SI - s0) * qt_bytes;
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int c = c0 + 32 * i;
+        for (int i = 0; i < 2; ++i) {
+          const int c = cb + 32 * i;
           if (c < qc16) *reinterpret_cast<uint4*>(t + c * 128 + ((q ^ (c & 7)) << 4)) = shift_window<SI - S / 2>(win[i]);
         }
       }
-      ShiftCols<S, SI + 1>::run(win, qc16, tid, dst, qt_bytes, s0, ns);
+      ShiftCols<S, SI + 1>::run(win, cb, qc16, q, dst, qt_bytes, s0, ns);
     }
   }
 };
 
 template <int S, int QC>
 __global__ void __launch_bounds__(WT_THREADS, 1)
-wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constant__ CUtensorMap tmap_q, const WtParams p) {
+wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constant__ CUtensorMap tmap_q,
+                 const __grid_constant__ WtParams p) {
   constexpr bool SHIFT = S > 1;
-  constexpr int NT = 128 / QC;
+  constexpr int NT = 256 / QC;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int qblk_bytes = p.ns * p.qt_bytes;                 // the shifted tiles of one 64-pixel block of a Q row
+  const int qblk_bytes = p.ns_max * p.qt_bytes;             // the shifted tiles of one 64-pixel block of a Q row
   const int qrow_bytes = p.nbw * qblk_bytes;                // ... of a whole strip row
   const int prow_bytes = p.nbw * p.p_blk;
   const int rawrow_bytes = p.nbw * p.raw_bytes;
@@ -134,25 +142,32 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
   }
   __syncthreads();
 
-  // item -> (image n, column strip, row range [ha, hb))
+  // item -> (image n, column strip, row range [ha, hb), tap rectangle = pass)
 #define WT_ITEM(it)                                                               \
-  const int sp_ = (it) % p.row_splits;                                            \
-  const int strip_ = ((it) / p.row_splits) % p.strips;                            \
-  const int n_ = (it) / (p.row_splits * p.strips);                                \
+  const int pass_ = (it) % p.npass, rest_ = (it) / p.npass;                       \
+  const int sp_ = rest_ % p.row_splits;                                           \
+  const int strip_ = (rest_ / p.row_splits) % p.strips;                           \
+  const int n_ = rest_ / (p.row_splits * p.strips);                               \
+  const int r0 = p.rect[pass_][0], nr = p.rect[pass_][1];                         \
+  const int s0 = p.rect[pass_][2], ns = p.rect[pass_][3];                         \
   const int w0 = strip_ * 64 * p.nbw;                                             \
   const int ha = sp_ * p.rows_per_split, hb = min(p.H, ha + p.rows_per_split);    \
   const int rows = hb - ha;                                                       \
-  const int q_first = ha + p.r0 - p.ph;   /* image row of Q ring row 0 */         \
-  const int q_rows = rows + p.nr - 1;
+  const int q_first = ha + r0 - p.ph;   /* image row of Q ring row 0 */           \
+  const int q_rows = rows + nr - 1;
 
-  if (warp == 0) {
+  // 640 x 96 registers at launch; the consumers' <= 128 accumulators need more: 24 + 2 x 56 + 2 x 168 <= 480.  Each
+  // role sets its count at the top of its own branch, so that ptxas allocates that branch at that count.
+  if (warp < 4) {
+    setmaxnreg_dec<24>();
     // ================= producer =================
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       tma_prefetch_desc(&tmap_p);
       tma_prefetch_desc(&tmap_q);
       Ring qr, pr, rr;     // Q ring rows / P rows / raw rows issued so far (global counters across items)
       for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
         WT_ITEM(it)
+        (void)s0; (void)ns;
         if (rows <= 0) continue;
         for (int i = 0; i < q_rows; ++i) {
           if (SHIFT) {
@@ -170,8 +185,8 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
               tma_load_4d(qt_base + s * qrow_bytes + b * qblk_bytes, &tmap_q, &qt_full[s], w0 + 64 * b, q_first + i, 0, n_);
             ++qr.i;
           }
-          if (i >= p.nr - 1) {     // P row of step j = i - (nr - 1)
-            const int j = i - (p.nr - 1);
+          if (i >= nr - 1) {     // P row of step j = i - (nr - 1)
+            const int j = i - (nr - 1);
             const int s = pr.slot(p.psn);
             mbar_wait(&p_empty[s], pr.phase(p.psn) ^ 1);
             mbar_arrive_expect_tx(&p_full[s], p.nbw * p.p_bytes);
@@ -183,6 +198,7 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
       }
     }
   } else if (warp >= 12) {
+    setmaxnreg_dec<56>();
     // ================= shifter: raw Q row -> S' shifted K-major tiles =================
     if (SHIFT) {
       const int tid = threadIdx.x - 12 * 32;
@@ -198,24 +214,29 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
           const int qs = qr.slot(p.rq);
           for (int b = 0; b < p.nbw; ++b) {
             const uint8_t* raw = raw_base + rs * rawrow_bytes + b * p.raw_bytes;
-            uint32_t win[4][8];
+            // channels c0 + 32 k, k < 4, in two halves: 16 registers of windows at a time (the shifter has 56)
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const int c = c0 + 32 * k;
-              if (c < p.Qc16) {   // warp-uniform (4 consecutive channels per warp, Qc16 multiple of 16)
-                const uint8_t* row = raw + c * RAW_ROW;
-                const uint4 own = *reinterpret_cast<const uint4*>(row + 16 * (q + 1));
-                uint32_t lz = __shfl_up_sync(0xffffffffu, own.z, 1), lw = __shfl_up_sync(0xffffffffu, own.w, 1);
-                uint32_t rx = __shfl_down_sync(0xffffffffu, own.x, 1), ry = __shfl_down_sync(0xffffffffu, own.y, 1);
-                if (q == 0) { const uint2 h = *reinterpret_cast<const uint2*>(row + 8); lz = h.x; lw = h.y; }
-                if (q == 7) { const uint2 h = *reinterpret_cast<const uint2*>(row + 16 * 9); rx = h.x; ry = h.y; }
-                win[k][0] = lz; win[k][1] = lw; win[k][2] = own.x; win[k][3] = own.y;
-                win[k][4] = own.z; win[k][5] = own.w; win[k][6] = rx; win[k][7] = ry;
+            for (int hf = 0; hf < 2; ++hf) {
+              const int cb = c0 + 64 * hf;
+              uint32_t win[2][8];
+#pragma unroll
+              for (int k = 0; k < 2; ++k) {
+                const int c = cb + 32 * k;
+                if (c < p.Qc16) {   // warp-uniform (4 consecutive channels per warp, Qc16 multiple of 16)
+                  const uint8_t* row = raw + c * RAW_ROW;
+                  const uint4 own = *reinterpret_cast<const uint4*>(row + 16 * (q + 1));
+                  uint32_t lz = __shfl_up_sync(0xffffffffu, own.z, 1), lw = __shfl_up_sync(0xffffffffu, own.w, 1);
+                  uint32_t rx = __shfl_down_sync(0xffffffffu, own.x, 1), ry = __shfl_down_sync(0xffffffffu, own.y, 1);
+                  if (q == 0) { const uint2 h = *reinterpret_cast<const uint2*>(row + 8); lz = h.x; lw = h.y; }
+                  if (q == 7) { const uint2 h = *reinterpret_cast<const uint2*>(row + 16 * 9); rx = h.x; ry = h.y; }
+                  win[k][0] = lz; win[k][1] = lw; win[k][2] = own.x; win[k][3] = own.y;
+                  win[k][4] = own.z; win[k][5] = own.w; win[k][6] = rx; win[k][7] = ry;
+                }
               }
+              if (b == p.nbw - 1 && hf == 1) mbar_arrive(&raw_empty[rs]);       // the whole raw row has been read
+              if (b == 0 && hf == 0) mbar_wait(&qt_empty[qs], qr.phase(p.rq) ^ 1);
+              ShiftCols<S, 0>::run(win, cb, p.Qc16, q, qt_base + qs * qrow_bytes + b * qblk_bytes, p.qt_bytes, s0, ns);
             }
-            if (b == p.nbw - 1) mbar_arrive(&raw_empty[rs]);       // the whole raw row has been read
-            if (b == 0) mbar_wait(&qt_empty[qs], qr.phase(p.rq) ^ 1);
-            ShiftCols<S, 0>::run(win, p.Qc16, tid, qt_base + qs * qrow_bytes + b * qblk_bytes, p.qt_bytes, p.s0, p.ns);
           }
           ++rr.i;
           fence_proxy_async();
@@ -224,22 +245,23 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
         }
       }
     }
-  } else if (threadIdx.x >= 128) {
+  } else {
+    setmaxnreg_inc<168>();
     // ================= consumers: wgmma over (row step, 64-pixel block, tap), then fp32 atomics on dW =================
     const int wg = (threadIdx.x >> 7) - 1;
     const int w4 = (threadIdx.x >> 5) & 3;
     const bool wg_lead = (threadIdx.x & 127) == 0;
-    const int ntaps = p.nr * p.ns;
     float acc[NT][QC / 2];
     Ring qr, pr;          // qr.i = ring index of Q row 0 of the current item
     for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
       WT_ITEM(it)
       (void)w0; (void)n_; (void)q_first;
       if (rows <= 0) continue;
+      const int ntaps = nr * ns;
       int rel_p = -1, rel_q = -1;             // slots read by the last committed wgmma group
       for (int j = 0; j < rows; ++j) {
         // Q rows j .. j + nr - 1 must have landed: all of them at the first step, then one new row per step
-        for (int i = (j == 0 ? 0 : p.nr - 1); i < p.nr; ++i) {
+        for (int i = (j == 0 ? 0 : nr - 1); i < nr; ++i) {
           const int g = qr.i + j + i;
           mbar_wait(&qt_full[g % p.rq], (g / p.rq) & 1);
         }
@@ -250,8 +272,8 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
           const uint32_t sa = smem_u32(p_base + ps * prow_bytes + b * p.p_blk) + wg * 8192;
 #pragma unroll
           for (int a = 0; a < NT; ++a) {
-            const int ta = min(a, ntaps - 1);
-            const int r = ta / p.ns, si = ta - r * p.ns;
+            if (a >= ntaps) break;              // warp-uniform: a pass with fewer taps skips its spare accumulators
+            const int r = a / ns, si = a - r * ns;
             const int g = qr.i + j + r;
             const uint32_t sq = smem_u32(qt_base + (g % p.rq) * qrow_bytes + b * qblk_bytes + si * p.qt_bytes);
 #pragma unroll
@@ -283,7 +305,7 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
 #pragma unroll
       for (int a = 0; a < NT; ++a) {
         if (a < ntaps) {
-          int r = p.r0 + a / p.ns, s = p.s0 + a % p.ns;
+          int r = r0 + a / ns, s = s0 + a % ns;
           if (p.modeB) { r = p.R - 1 - r; s = p.S - 1 - s; }
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
@@ -328,9 +350,8 @@ int launch_wt(const CUtensorMap& tp, const CUtensorMap& tq, const WtParams& p, i
   return SPC_OK;
 }
 
-// tap rectangles ("passes") of an R x S filter whose accumulators fit the registers; returns the count (0: unsupported)
-int plan_passes(int R, int S, int Qc16, int (*rect)[4]) {
-  const int maxt = 128 / Qc16;          // taps per pass: the kernel's NT
+// tap rectangles ("passes") of an R x S filter at most maxt taps each; returns the count (0: no plan)
+int plan_passes(int R, int S, int maxt, int (*rect)[4]) {
   if (maxt < 1) return 0;
   int n = 0;
   if (R * S <= maxt) { rect[n][0] = 0; rect[n][1] = R; rect[n][2] = 0; rect[n][3] = S; return 1; }
@@ -355,9 +376,11 @@ bool wgrad_tap_supported(int K, int C, int R, int S, int H, int W, int stride) {
   // 1.4x faster than the line buffer there (profiles/r2_tap_probe_v2d.txt) -- it keeps those shapes
   if (!(S == 3 || S == 5 || S == 7) || (R & 1) == 0 || R > 7) return false;
   if (K > 128 || C > 128) return false;
+  // the shapes this kernel serves are those with a plan of 128 / QC taps per pass, the set it was measured on
+  // against the shifted-copy path; it runs them in passes of up to 256 / QC taps
   const int Qc16 = rup(K >= C ? C : K, 16);
-  int rect[16][4];
-  return plan_passes(R, S, Qc16, rect) > 0;
+  int rect[MAXPASS][4];
+  return plan_passes(R, S, 128 / Qc16, rect) > 0;
 }
 
 // dw += wgrad(x [N][C][H][W], dy [N][K][H][W]) over the zero-padded tile (pad = (R-1)/2, (S-1)/2), bf16 inputs
@@ -375,9 +398,14 @@ int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, in
   p.raw_bytes = p.Qc16 * RAW_ROW;
   const __nv_bfloat16* P = p.modeB ? x : dy;
   const __nv_bfloat16* Q = p.modeB ? dy : x;
-  int rect[16][4];
-  const int npass = plan_passes(R, S, p.Qc16, rect);
-  SPC_REQUIRE(npass > 0, "wgrad_tap: %dx%d filter with %d Q channels does not fit the accumulators", R, S, p.Qch);
+  const int npass = plan_passes(R, S, 256 / p.Qc16, p.rect);   // NT = 256 / QC taps per pass
+  SPC_REQUIRE(npass > 0 && npass <= MAXPASS, "wgrad_tap: %dx%d filter with %d Q channels does not fit the accumulators",
+              R, S, p.Qch);
+  p.npass = npass;
+  for (int pi = 0; pi < npass; ++pi) {
+    p.nr_max = max(p.nr_max, p.rect[pi][1]);
+    p.ns_max = max(p.ns_max, p.rect[pi][3]);
+  }
   CUtensorMap tp, tq;
   {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)p.Pch, (uint64_t)N};
@@ -401,52 +429,48 @@ int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, in
     while (p.nbw < 4 && rowb * p.nbw < 12 * 1024 && W % (128 * p.nbw) == 0) p.nbw *= 2;
   }
   p.strips = W / (64 * p.nbw);
-  for (int pi = 0; pi < npass; ++pi) {
-    // mode B mirrors the tap indices: the rectangle is planned in the kernel's (mirrored) index space either way
-    p.r0 = rect[pi][0]; p.nr = rect[pi][1]; p.s0 = rect[pi][2]; p.ns = rect[pi][3];
-    const int qrow_bytes = p.nbw * p.ns * p.qt_bytes, prow = p.nbw * p.p_blk, rawrow = S > 1 ? p.nbw * p.raw_bytes : 0;
-    // ring depths.  Rows of many channels (>= ~12 KB per strip row) keep enough bytes in flight with 3 P stages,
-    // 2 raw rows and nr + 3 shifted rows (measured: deeper rings cost 10 % there); small rows are latency-bound
-    // on the ~2 us L2 round trip of their TMA loads, so they take whatever depth fits.
-    const bool small_rows = prow + p.nbw * p.qt_bytes < 12 * 1024;
-    p.psn = 3; p.rawn = S > 1 ? 2 : 0; p.rq = p.nr + 1;
-    int rem = WT_SMEM_LIMIT - WT_SMEM_AUX - p.psn * prow - p.rawn * rawrow - p.rq * qrow_bytes;
-    SPC_REQUIRE(rem >= 0, "wgrad_tap: shared memory too small (rows %d, %d bytes per row)", p.nr, qrow_bytes);
-    if (small_rows) {
-      for (bool grew = true; grew;) {
-        grew = false;
-        if (S > 1 && p.rawn < MAXRAW && rem >= rawrow) { ++p.rawn; rem -= rawrow; grew = true; }
-        if (p.psn < MAXP && rem >= prow) { ++p.psn; rem -= prow; grew = true; }
-        if (p.rq < MAXQ && p.rq < p.nr + 8 && rem >= qrow_bytes) { ++p.rq; rem -= qrow_bytes; grew = true; }
-      }
-    } else {
-      while (p.rq < p.nr + 3 && p.rq < MAXQ && rem >= qrow_bytes) { ++p.rq; rem -= qrow_bytes; }
+  // mode B mirrors the tap indices: the rectangles are planned in the kernel's (mirrored) index space either way
+  const int qrow_bytes = p.nbw * p.ns_max * p.qt_bytes, prow = p.nbw * p.p_blk, rawrow = S > 1 ? p.nbw * p.raw_bytes : 0;
+  // ring depths.  Rows of many channels (>= ~12 KB per strip row) keep enough bytes in flight with 3 P stages,
+  // 2 raw rows and nr + 3 shifted rows (measured: deeper rings cost 10 % there); small rows are latency-bound
+  // on the ~2 us L2 round trip of their TMA loads, so they take whatever depth fits.
+  const bool small_rows = prow + p.nbw * p.qt_bytes < 12 * 1024;
+  p.psn = 3; p.rawn = S > 1 ? 2 : 0; p.rq = p.nr_max + 1;
+  int rem = WT_SMEM_LIMIT - WT_SMEM_AUX - p.psn * prow - p.rawn * rawrow - p.rq * qrow_bytes;
+  SPC_REQUIRE(rem >= 0, "wgrad_tap: shared memory too small (rows %d, %d bytes per row)", p.nr_max, qrow_bytes);
+  if (small_rows) {
+    for (bool grew = true; grew;) {
+      grew = false;
+      if (S > 1 && p.rawn < MAXRAW && rem >= rawrow) { ++p.rawn; rem -= rawrow; grew = true; }
+      if (p.psn < MAXP && rem >= prow) { ++p.psn; rem -= prow; grew = true; }
+      if (p.rq < MAXQ && p.rq < p.nr_max + 8 && rem >= qrow_bytes) { ++p.rq; rem -= qrow_bytes; grew = true; }
     }
-    // row splits: fill the persistent grid with whole waves of (image, strip, row range) items
-    const int base_items = N * p.strips;
-    int best = 1;
-    double best_eff = 0.0;
-    for (int sp = 1; sp <= 64 && H / sp >= 8 * p.nr; ++sp) {
-      const int items = base_items * sp, waves = (items + sms - 1) / sms;
-      if (waves > 3) break;
-      const double eff = (double)items / ((double)waves * sms) * (1.0 - (double)(p.nr - 1) * sp / (H + (p.nr - 1) * sp));
-      if (eff > best_eff + 1e-9) { best_eff = eff; best = sp; }
-    }
-    p.row_splits = best;
-    p.rows_per_split = (H + best - 1) / best;
-    p.num_items = base_items * best;
-    const int smem = p.psn * prow + p.rq * qrow_bytes + p.rawn * rawrow + WT_SMEM_AUX;
-    int rc = SPC_EUNSUPPORTED;
-    set_error("wgrad_tap: unsupported filter width %d / %d Q channels", S, p.Qc16);
-#define WT_CASE(s, qc) if (S == s && p.Qc16 == qc) rc = launch_wt<s, qc>(tp, tq, p, smem, st);
+  } else {
+    while (p.rq < p.nr_max + 3 && p.rq < MAXQ && rem >= qrow_bytes) { ++p.rq; rem -= qrow_bytes; }
+  }
+  // row splits: fill the persistent grid with whole waves of (image, strip, row range, pass) items
+  const int base_items = N * p.strips * npass;
+  int best = 1;
+  double best_eff = 0.0;
+  for (int sp = 1; sp <= 64 && H / sp >= 8 * p.nr_max; ++sp) {
+    const int items = base_items * sp, waves = (items + sms - 1) / sms;
+    if (waves > 3) break;
+    const double eff = (double)items / ((double)waves * sms) *
+                       (1.0 - (double)(p.nr_max - 1) * sp / (H + (p.nr_max - 1) * sp));
+    if (eff > best_eff + 1e-9) { best_eff = eff; best = sp; }
+  }
+  p.row_splits = best;
+  p.rows_per_split = (H + best - 1) / best;
+  p.num_items = base_items * best;
+  const int smem = p.psn * prow + p.rq * qrow_bytes + p.rawn * rawrow + WT_SMEM_AUX;
+#define WT_CASE(s, qc) if (S == s && p.Qc16 == qc) return launch_wt<s, qc>(tp, tq, p, smem, st);
 #define WT_CASES(s) WT_CASE(s, 16) WT_CASE(s, 32) WT_CASE(s, 48) WT_CASE(s, 64) WT_CASE(s, 80) WT_CASE(s, 96) \
                     WT_CASE(s, 112) WT_CASE(s, 128)
-    WT_CASES(3) WT_CASES(5) WT_CASES(7)
+  WT_CASES(3) WT_CASES(5) WT_CASES(7)
 #undef WT_CASES
 #undef WT_CASE
-    if (rc) return rc;
-  }
-  return SPC_OK;
+  set_error("wgrad_tap: unsupported filter width %d / %d Q channels", S, p.Qc16);
+  return SPC_EUNSUPPORTED;
 }
 
 }  // namespace spc
