@@ -35,7 +35,17 @@ extern "C" {
 enum { SPC_OK = 0, SPC_EINVAL = -1, SPC_ECUDA = -2, SPC_EUNSUPPORTED = -3, SPC_ENOMEM = -4 };
 enum { SPC_F32 = 0, SPC_BF16 = 1 };             /* storage dtype of x / w / y; accumulation is fp32 */
 enum { SPC_POOL_MAX = 0, SPC_POOL_AVG = 1 };
-enum { SPC_ALGO_AUTO = 0, SPC_ALGO_DIRECT = 1, SPC_ALGO_TCGEN05 = 2 };
+/* SPC_ALGO_TF32: like AUTO, but fp32 storage may use the TF32 tensor cores (fp32 accumulation) where the shape
+ * qualifies: 1x1 filters, stride 1 or 2, on the shapes the bf16 1x1 path takes (H*W / stride^2 a multiple of 8;
+ * stride 2 also needs even H and W % 32 == 0).  Every other fp32 shape (multi-tap filters, misaligned pixel counts)
+ * runs on the direct kernels as with AUTO, and bf16 behaves exactly as with AUTO.  Rounding: fprop and dgrad round
+ * both operands (x or dy, and w) to tf32 (10 fraction bits) to nearest; wgrad feeds dy and x to the tensor cores
+ * unconverted, which use the top 19 bits of each word, i.e. truncate them.  Products are exact and summed in fp32.
+ * Error bound per element, with A = the same operation on |x|, |w|, |dy| (and |b|) in exact arithmetic:
+ *   inputs already tf32-representable:  |got - exact| <= 2^-12 A
+ *   arbitrary fp32 inputs:              |got - exact| <= (2^-9 + 2^-12) A
+ * SPC_ALGO_TCGEN05 still rejects fp32 (SPC_EUNSUPPORTED). */
+enum { SPC_ALGO_AUTO = 0, SPC_ALGO_DIRECT = 1, SPC_ALGO_TCGEN05 = 2, SPC_ALGO_TF32 = 3 };
 
 /* Geometry of one spatially-partitioned convolution on one tile.
  * Mirrors conv_spatial.__init__ (spatial.py:26-155): padding is "same"

@@ -5,6 +5,7 @@
 // receptive field reaches into a halo are then recomputed by a small GEMM over just those
 // outputs, which reads the received strips in place.  Interior compute therefore never waits on
 // the halo exchange -- the overlap the reference left as dead code (spatial.py:415-866).
+// fp32 runs there only with SPC_ALGO_TF32, and only its 1x1 layers (gemm_tf32.cu, which have no halo).
 // Everything else runs entirely on the direct kernel; when its interior and boundary passes are
 // split (spc_conv2d_fwd_interior / _boundary, fp32 or SPC_ALGO_DIRECT), it recomputes the strips.
 #include "common.cuh"
@@ -150,12 +151,15 @@ void spc_conv_out_shape(const spc_conv_desc* d, int* Ho, int* Wo) {
 
 int spc_conv_uses_tcgen05(const spc_conv_desc* d, int op) {
   if (!d || d->algo == SPC_ALGO_DIRECT) return 0;
+  // fp32 storage reaches the tensor cores only when the caller opts in to TF32 (gemm_tf32.cu)
+  if (d->dtype == SPC_F32) return (d->algo == SPC_ALGO_TF32 && tf32_supported(d)) ? 1 : 0;
   return tc_supported(d, op) ? 1 : 0;
 }
 
 size_t spc_conv_workspace_bytes(const spc_conv_desc* d, int op) {
   if (!d) return 0;
-  return spc_conv_uses_tcgen05(d, op) ? tc_workspace_bytes(d, op) : 0;
+  if (!spc_conv_uses_tcgen05(d, op)) return 0;
+  return d->dtype == SPC_F32 ? tf32_workspace_bytes(d, op) : tc_workspace_bytes(d, op);
 }
 
 // Boundary strips: output rows / columns whose window reaches outside the tile, recomputed from
@@ -180,6 +184,7 @@ static int fwd_interior(const spc_conv_desc* d, const void* x, const void* w, co
     set_error("conv_fwd: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
     return SPC_EUNSUPPORTED;
   }
+  if (tc && d->dtype == SPC_F32) return tf32_conv_fwd(d, x, w, bias, y, workspace, workspace_bytes, st);
   if (tc) return tc_conv_fwd(d, x, w, bias, y, workspace, workspace_bytes, st);
   return launch_conv_direct(fwd_params(d, x, nullptr, w, bias, y), d->dtype, st);
 }
@@ -228,6 +233,7 @@ int spc_conv2d_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void
     set_error("conv_dgrad: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
     return SPC_EUNSUPPORTED;
   }
+  if (tc && d->dtype == SPC_F32) return tf32_conv_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
   if (tc) return tc_conv_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
 
   int Ho, Wo;
@@ -288,7 +294,11 @@ int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo
     set_error("conv_wgrad: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
     return SPC_EUNSUPPORTED;
   }
-  if (tc) {
+  if (tc && d->dtype == SPC_F32) {
+    // 1x1 only: no output window reaches a halo strip, so there is nothing to add for the strips
+    rc = tf32_conv_wgrad(d, x, dy, dw, workspace, workspace_bytes, st);
+    if (rc) return rc;
+  } else if (tc) {
     rc = tc_conv_wgrad(d, x, dy, dw, /*accumulate=*/1, workspace, workspace_bytes, st);
     if (rc) return rc;
     // add the halo pixels' contribution (exact by linearity): boundary GEMM over the outputs whose windows reach a strip

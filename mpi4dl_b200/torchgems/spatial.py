@@ -17,6 +17,7 @@ libspconv.so loads.
 """
 import ctypes as C
 import math
+import os
 
 import torch
 import torch.distributed as dist
@@ -49,6 +50,12 @@ def _workspace(nbytes, device):
 
 def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(None)
+
+
+def conv_algo_default():
+    """Initial value of a conv layer's `algo`: SPCONV_ALLOW_TF32=1 lets the fp32 1x1 convolutions run on the TF32
+    tensor cores (SPC_ALGO_TF32: 10-bit mantissa products, fp32 sums; bf16 is unaffected), else SPC_ALGO_AUTO."""
+    return _lib.SPC_ALGO_TF32 if os.environ.get("SPCONV_ALLOW_TF32", "0") == "1" else _lib.SPC_ALGO_AUTO
 
 
 class _SpatialTopology:
@@ -344,7 +351,7 @@ class conv_spatial(nn.Conv2d, _SpatialTopology):
             self.halo_len_height_d2, self.halo_len_width_d2 = 0, 0
             self.neighbours = None          # never exchanges
         self.set_tags()
-        self.algo = _lib.SPC_ALGO_AUTO
+        self.algo = conv_algo_default()
         # a plain attribute (not a parameter / buffer: state_dict keys stay the reference's), flippable per layer
         self.exact_backward = halo_transport.exact_backward_default()
 
@@ -590,7 +597,7 @@ class local_conv2d(nn.Conv2d):
             assert p_ in (0, s_), "local_conv2d: padding must be 0 or (k-1)//2"
         assert tuple(self.padding) == self._same or tuple(self.stride) == (1, 1), \
             "local_conv2d: a valid (padding=0) convolution is supported for stride 1 only"
-        self.algo = _lib.SPC_ALGO_AUTO
+        self.algo = conv_algo_default()
 
     def forward(self, tensor):
         _require_cuda(tensor, "local_conv2d")
