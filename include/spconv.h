@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define SPC_VERSION 100
+#define SPC_VERSION 101
 
 enum { SPC_OK = 0, SPC_EINVAL = -1, SPC_ECUDA = -2, SPC_EUNSUPPORTED = -3, SPC_ENOMEM = -4 };
 enum { SPC_F32 = 0, SPC_BF16 = 1 };             /* storage dtype of x / w / y; accumulation is fp32 */
@@ -132,18 +132,28 @@ int spc_pool2d_bwd(const spc_pool_desc* d, const void* x, const spc_halo* halo, 
  * The cells of the spatial stages chain ReLU -> conv -> nn.BatchNorm2d (models/amoebanet.py:365-398 of the
  * reference) / BatchNorm2d -> ReLU -> conv (resnet_spatial.py:165-180) as separate eager kernels; statistics
  * are over the LOCAL tile only (SURVEY 8a N4).  These four entry points do normalisation + the following ReLU
- * in one HBM pass each way.  y, z, dz, dy: [N][C][H*W] (NCHW, H*W % 8 == 0), dtype SPC_F32 | SPC_BF16;
- * all per-channel vectors are fp32 device arrays of C elements.
- *   spc_bn_stats     : sum[c] = sum y, sumsq[c] = sum y^2                          (replaces the statistics pass)
+ * in one HBM pass each way.  y, z, dz, dy: [N][C][H*W] (NCHW, H*W % 8 == 0), dtype SPC_F32 | SPC_BF16, 16-byte aligned;
+ * all per-channel vectors are fp32 device arrays of C elements, 4-byte aligned.  A misaligned pointer is SPC_EINVAL.
+ *   spc_bn_stats     : mean[c] = sum y / M, var[c] = sum (y - mean)^2 / M (biased), M = N*H*W (replaces the statistics pass)
  *   spc_bn_apply     : z = relu?((y - mean[c]) * rstd[c] * gamma[c] + beta[c])     (BN apply + nn.ReLU)
  *   spc_bn_bwd_reduce: dsum[c] = sum g, dsumx[c] = sum g * xhat, g = dz * [z > 0]  (= dbeta, dgamma)
- *   spc_bn_bwd_apply : dy = gamma * rstd * (g - dsum/M - xhat * dsumx/M), M = N*H*W */
-int spc_bn_stats(int N, int C, long long HW, int dtype, const void* y, float* sum, float* sumsq, void* stream);
+ *   spc_bn_bwd_apply : dy = gamma * rstd * (g - dsum/M - xhat * dsumx/M)
+ * spc_bn_stats and spc_bn_bwd_reduce write one partial per (plane, 16384-element chunk) to `workspace`
+ * (spc_bn_workspace_bytes(N, C, HW) bytes, 16-byte aligned) and merge each channel's partials in a fixed order in fp64:
+ * no floating-point atomics, every output of the four entry points is bit-reproducible.  Error bounds per channel,
+ * against exact arithmetic on the stored y (and the same mean, rstd, gamma, beta for the backward sums):
+ *   |mean - exact| <= 2^-23 |exact mean| + 2^-19 mean|y - exact mean|
+ *   |var - exact|  <= 2^-16 exact var + 2^-30 mean(y^2)
+ *   |dsum - exact| <= 2^-19 sum|g|,   |dsumx - exact| <= 2^-19 sum|g * xhat|
+ * (tests/test_bnrelu_bounds.py derives these and the per-element bounds of z and dy). */
+size_t spc_bn_workspace_bytes(int N, int C, long long HW);   /* 0 for an invalid shape */
+int spc_bn_stats(int N, int C, long long HW, int dtype, const void* y, float* mean, float* var, void* workspace,
+                 size_t workspace_bytes, void* stream);
 int spc_bn_apply(int N, int C, long long HW, int dtype, const void* y, const float* mean, const float* rstd,
                  const float* gamma, const float* beta, int relu, void* z, void* stream);
 int spc_bn_bwd_reduce(int N, int C, long long HW, int dtype, const void* dz, const void* y, const float* mean,
                       const float* rstd, const float* gamma, const float* beta, int relu, float* dsum,
-                      float* dsumx, void* stream);
+                      float* dsumx, void* workspace, size_t workspace_bytes, void* stream);
 int spc_bn_bwd_apply(int N, int C, long long HW, int dtype, const void* dz, const void* y, const float* mean,
                      const float* rstd, const float* gamma, const float* beta, int relu, const float* dsum,
                      const float* dsumx, void* dy, void* stream);

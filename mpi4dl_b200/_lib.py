@@ -43,9 +43,11 @@ SYMBOLS = [
     ("spc_conv_out_shape", None, [C.POINTER(ConvDesc), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     ("spc_pool2d_fwd", C.c_int, [C.POINTER(PoolDesc), _P, C.POINTER(Halo), _P, _P]),
     ("spc_pool2d_bwd", C.c_int, [C.POINTER(PoolDesc), _P, C.POINTER(Halo), _P, _P, _P]),
-    ("spc_bn_stats", C.c_int, [C.c_int, C.c_int, C.c_longlong, C.c_int, _P, _P, _P, _P]),
+    ("spc_bn_workspace_bytes", C.c_size_t, [C.c_int, C.c_int, C.c_longlong]),
+    ("spc_bn_stats", C.c_int, [C.c_int, C.c_int, C.c_longlong, C.c_int, _P, _P, _P, _P, C.c_size_t, _P]),
     ("spc_bn_apply", C.c_int, [C.c_int, C.c_int, C.c_longlong, C.c_int, _P, _P, _P, _P, _P, C.c_int, _P, _P]),
-    ("spc_bn_bwd_reduce", C.c_int, [C.c_int, C.c_int, C.c_longlong, C.c_int, _P, _P, _P, _P, _P, _P, C.c_int, _P, _P, _P]),
+    ("spc_bn_bwd_reduce", C.c_int, [C.c_int, C.c_int, C.c_longlong, C.c_int, _P, _P, _P, _P, _P, _P, C.c_int, _P, _P, _P,
+                                    C.c_size_t, _P]),
     ("spc_bn_bwd_apply", C.c_int, [C.c_int, C.c_int, C.c_longlong, C.c_int, _P, _P, _P, _P, _P, _P, C.c_int, _P, _P, _P, _P]),
     ("spc_halo_pack", C.c_int, [C.c_int] * 7 + [_P, C.POINTER(_P * 9), _P]),
     ("spc_halo_pad", C.c_int, [C.c_int] * 7 + [_P, C.POINTER(Halo), _P, _P]),

@@ -7,7 +7,8 @@ unbiased for running_var, momentum update of the running buffers -- and, when as
 in the chain, in one pass over HBM each way instead of three (stats, apply, relu) / five (backward).
 `relu_conv_bn_chain` is the drop-in forward for the  [ReLU, conv, BN] * k  Sequential of a spatial cell: same
 submodules, same state-dict keys, same numerics up to rounding (the BN output feeding a ReLU is rounded once, not
-twice).  Eval mode, non-CUDA tensors and H*W not a multiple of 8 take the module's own PyTorch path.
+twice).  Eval mode, non-CUDA tensors, H*W not a multiple of 8 and misaligned views take the module's own
+PyTorch path.
 """
 import ctypes as C
 
@@ -26,6 +27,13 @@ def _st():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def _workspace(L, N, Cc, HW, device):
+    """per-(plane, chunk) partials of spc_bn_stats / spc_bn_bwd_reduce"""
+    n = L.spc_bn_workspace_bytes(N, Cc, HW)
+    ws = torch.empty(n, dtype=torch.uint8, device=device)
+    return ws, C.c_void_p(ws.data_ptr()), n
+
+
 class _BnReluFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, y, gamma, beta, eps, relu, stats_out):
@@ -34,11 +42,11 @@ class _BnReluFn(torch.autograd.Function):
         N, Cc, H, W = y.shape
         HW = H * W
         code = _lib.dtype_code(y.dtype)
-        s = torch.empty(2, Cc, dtype=torch.float32, device=y.device)
-        _lib.check(L.spc_bn_stats(N, Cc, HW, code, _p(y), _p(s[0]), _p(s[1]), _st()), "spc_bn_stats")
+        st = torch.empty(2, Cc, dtype=torch.float32, device=y.device)
+        mean, var = st[0], st[1]                                   # var: biased (normalisation)
+        ws, wsp, nws = _workspace(L, N, Cc, HW, y.device)
+        _lib.check(L.spc_bn_stats(N, Cc, HW, code, _p(y), _p(mean), _p(var), wsp, nws, _st()), "spc_bn_stats")
         m = float(N * HW)
-        mean = s[0] / m
-        var = (s[1] / m - mean * mean).clamp_(min=0.0)            # biased variance (normalisation)
         rstd = torch.rsqrt(var + eps)
         g32 = gamma.detach().float().contiguous() if gamma is not None else torch.ones(Cc, device=y.device)
         b32 = beta.detach().float().contiguous() if beta is not None else torch.zeros(Cc, device=y.device)
@@ -57,12 +65,15 @@ class _BnReluFn(torch.autograd.Function):
         L = _lib.lib()
         y, mean, rstd, g32, b32 = ctx.saved_tensors
         dz = dz.contiguous()
+        if dz.data_ptr() % 16:                                     # the kernels read 16-byte vectors
+            dz = dz.clone()
         N, Cc, H, W = y.shape
         HW = H * W
         code = _lib.dtype_code(y.dtype)
         d = torch.empty(2, Cc, dtype=torch.float32, device=y.device)
+        ws, wsp, nws = _workspace(L, N, Cc, HW, y.device)
         _lib.check(L.spc_bn_bwd_reduce(N, Cc, HW, code, _p(dz), _p(y), _p(mean), _p(rstd), _p(g32), _p(b32), int(ctx.relu),
-                                       _p(d[0]), _p(d[1]), _st()), "spc_bn_bwd_reduce")
+                                       _p(d[0]), _p(d[1]), wsp, nws, _st()), "spc_bn_bwd_reduce")
         dy = None
         if ctx.needs_input_grad[0]:
             dy = torch.empty_like(y)
@@ -74,8 +85,11 @@ class _BnReluFn(torch.autograd.Function):
 
 
 def fusable(x, bn):
+    """The kernels read and write 16-byte vectors: a contiguous view whose storage offset breaks that alignment (the
+    kernels would read it in place) takes the module's path."""
     return (isinstance(bn, nn.BatchNorm2d) and bn.training and x.is_cuda and x.dim() == 4 and
-            (x.shape[2] * x.shape[3]) % 8 == 0 and x.dtype in (torch.float32, torch.bfloat16) and x.numel() > 0)
+            (x.shape[2] * x.shape[3]) % 8 == 0 and x.dtype in (torch.float32, torch.bfloat16) and x.numel() > 0 and
+            (x.data_ptr() % 16 == 0 or not x.is_contiguous()))
 
 
 def bn_relu(x, bn, relu=False):

@@ -26,9 +26,10 @@ def test_library_exports_every_declared_symbol():
     assert bound == set(names)
 
 
-def test_version_and_structs():
+def test_version_101_and_structs():
+    """SPC_VERSION 101: spc_bn_stats returns mean and variance and, with spc_bn_bwd_reduce, takes a workspace"""
     L = _lib.lib()
-    assert L.spc_version() == 100
+    assert L.spc_version() == 101
     assert C.sizeof(_lib.ConvDesc) == 13 * 4
     assert C.sizeof(_lib.PoolDesc) == 9 * 4
     assert C.sizeof(_lib.Halo) == 9 * C.sizeof(C.c_void_p)
