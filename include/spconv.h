@@ -124,7 +124,9 @@ void   spc_conv_out_shape(const spc_conv_desc* d, int* Ho, int* Wo);
  * padding=0 on the explicitly zero-padded tile (so avg always divides by k*k and max sees 0 at
  * true image borders). */
 int spc_pool2d_fwd(const spc_pool_desc* d, const void* x, const spc_halo* halo, void* y, void* stream);
-/* dx = crop(pool backward); max routes to the first maximal element (ATen semantics). */
+/* dx = crop(pool backward); max routes to the first maximal element (ATen semantics).
+ * NaN follows ATen's max_pool2d too (`v > max || isnan(v)`): a window that holds a NaN pools to NaN in the
+ * forward, and its gradient goes to the NaN (the last one in row-major window order if there are several). */
 int spc_pool2d_bwd(const spc_pool_desc* d, const void* x, const spc_halo* halo, const void* dy,
                    void* dx, void* stream);
 

@@ -37,6 +37,20 @@ template <typename T> __device__ __forceinline__ T from_f32(float v);
 template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
 template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
 
+// Max pooling follows ATen's max_pool2d rule, `val > maxval || isnan(val)`: v replaces the running maximum m when it
+// is larger or NaN.  So a window holding a NaN pools to NaN, its gradient goes to the (last) NaN, and among tied
+// maxima the first one in row-major window order takes the gradient.  fmaxf would drop the NaN instead.
+// pool_max_takes is the argmax step of the backward kernels (the bitwise | keeps it one predicate, no branch);
+// pool_bwd_s2_vec_kernel applies the same rule unrolled for its 2x2 windows.
+__device__ __forceinline__ bool pool_max_takes(float v, float m) { return (v > m) | (v != v); }
+// The forward value: max.NaN is NaN when either operand is, so a fold over the window in any order gives ATen's value
+// in one instruction, as fmaxf did (only the NaN's payload may differ).
+__device__ __forceinline__ float pool_max(float m, float v) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(m), "f"(v));
+  return r;
+}
+
 // A tile plus its received halo strips, addressed in UNPADDED tile coordinates: h in
 // [-hh, H+hh), w in [-hw, W+hw).  Anything not covered by the tile or a non-NULL strip reads
 // as 0 -- this is ZeroPad2d + copy_halo_exchange_values (reference spatial.py:1020,405-413)

@@ -136,7 +136,7 @@ __global__ void __launch_bounds__(256) pool_halo_bwd_kernel(const PoolHaloParams
           for (int a = 0; a < p.k; ++a)
             for (int b = 0; b < p.k; ++b) {
               const float v = tile_load<T>(p.in, n, c, h0 + a, w0 + b);
-              if (v > best) { best = v; bi = a * p.k + b; }
+              if (pool_max_takes(v, best)) { best = v; bi = a * p.k + b; }
             }
           if (bi == (h - h0) * p.k + (w - w0)) g += to_f32<T>(dyp[(size_t)oy * p.Wo + ox]);
         }

@@ -93,17 +93,32 @@ def test_pool_strip_gradient(mode, st, dtype):
     L = _lib.lib()
     rng = np.random.default_rng(1)
     k, h = 3, 1
-    for name, rank, method, P in _masks():
+
+    def aten_bwd(xp, gy):
+        """ATen's pool backward on the padded tile in float64 (max: first maximum, NaN wins, the last of two NaNs)"""
+        xd = torch.tensor(xp, dtype=torch.float64, requires_grad=True)
+        y = torch.nn.functional.max_pool2d(xd, k, st) if mode == "max" else torch.nn.functional.avg_pool2d(xd, k, st)
+        return torch.autograd.grad(y, xd, gy)[0]
+
+    # random data; integers in {-2..2} (tied maxima, also with the zero pad); 4 % NaN, received strips included
+    for regime, (name, rank, method, P) in [(r, m) for r in ("normal", "ties", "nan") for m in _masks()]:
         H0, W0 = {"square": (36, 48), "vertical": (12, 48), "horizontal": (36, 16)}[method]
-        full = torch.tensor(rng.standard_normal((2, 8, H0, W0)).astype(np.float32)).to(dtype).float().numpy()
+        if regime == "ties":
+            full = rng.integers(-2, 3, (2, 8, H0, W0)).astype(np.float32)
+        else:
+            full = rng.standard_normal((2, 8, H0, W0)).astype(np.float32)
+            if regime == "nan":
+                full[rng.random(full.shape) < 0.04] = np.nan
+        full = torch.tensor(full).to(dtype).float().numpy()
         tiles = so.split(full, method, P)
         xp = so.exchange_halos(tiles, method, h, h)[rank]
         mask = so.neighbour_mask(method, P, rank)
         N, Cc, H, W = tiles[rank].shape
         Ho, Wo = (H + 2 * h - k) // st + 1, (W + 2 * h - k) // st + 1
         gy = torch.randn(N, Cc, Ho, Wo).to(dtype)
-        ref = torch.tensor(xo.pool_bwd64(xp, gy.double().numpy(), mode, k, st))
-        A = torch.tensor(xo.pool_bwd64(xp, gy.double().abs().numpy(), mode, k, st))
+        ref = aten_bwd(xp, gy.double())
+        A = aten_bwd(xp, gy.double().abs())
+        name = "%s %s" % (regime, name)
         x = torch.tensor(tiles[rank], dtype=dtype, device=DEV)
         strips = strips_from_padded(xp, mask, h, h, dtype)
         gyd = gy.to(DEV)

@@ -481,17 +481,41 @@ def run_boundary_direct(c, mask, tag, dtype, spc_dtype, algo):
     return k, lambda: traced(boundary)[1]
 
 
-@pytest.mark.parametrize("path", ["fixup"] + list(DIRECT_PATHS))
+def run_wgrad_direct(c, mask, tag):
+    """fp32 wgrad on the direct kernel, which reads the strips in place; dw, db against the fp64 reference with the
+    always-valid bound of an fp32 sum of N Ho Wo exact products: gamma(N Ho Wo + 1) A, u = 2^-24"""
+    x, w, b, dy, strips = make_inputs(c, mask)
+    ref, A = reference(x, w, b, dy, strips, c.stride)
+    x, w, dy, *strips = [t.to(DEV, torch.float32) if t is not None else None for t in (x, w, dy, *strips)]
+    d = desc(c, dtype=_lib.SPC_F32)
+    assert not _lib.lib().spc_conv_uses_tcgen05(C.byref(d), 2), tag
+    Ho, Wo = out_hw(c)
+    n = c.N * Ho * Wo + 1
+    gam = n * 2.0 ** -24 / (1 - n * 2.0 ** -24)
+    dw = torch.full(w.shape, float("nan"), device=DEV)
+    db = torch.full((c.K,), float("nan"), device=DEV) if c.bias else None
+    _, k = traced(lambda: run_wgrad(d, x, strips, dy, dw, db, 0))
+    _record(tag, "dw", k, check(dw, ref["dw"], A["dw"], 0.0, gam, tag + " dw"))
+    if c.bias:
+        check(db, ref["db"], A["db"], 0.0, gam, tag + " db")
+    return k, lambda: traced(lambda: run_wgrad(d, x, strips, dy, dw, db, 0))[1]
+
+
+@pytest.mark.parametrize("path", ["fixup"] + list(DIRECT_PATHS) + ["wgrad_direct_fp32"])
 @pytest.mark.parametrize("grid", GRIDS, ids=[g[0] for g in GRIDS])
 @pytest.mark.parametrize("c", MASK_CASES, ids=case_id)
 def test_halo_masks(c, grid, path):
     """corner, edge and interior tiles of a 3x3 grid and the end / middle tiles of 3-way slicing: the bf16 halo
-    fix-up on the boundary GEMM, and the forward fix-up on the direct kernel (fp32, bf16 with SPC_ALGO_DIRECT)"""
+    fix-up on the boundary GEMM, the forward fix-up on the direct kernel (fp32, bf16 with SPC_ALGO_DIRECT), and the fp32
+    wgrad on the direct kernel"""
     method, P = grid
     for mask in _masks(c, method, P):
         tag = "%s %s%s %s" % (case_id(c), method, "".join(map(str, mask)), path)
         fix = _fixup_expected(c, mask)
-        if path == "fixup":
+        if path == "wgrad_direct_fp32":
+            k, retrace = run_wgrad_direct(c, mask, tag)
+            assert launched(k, lambda k: "wgrad_direct_kernel" in _names(k), retrace), (tag, sorted(k))
+        elif path == "fixup":
             kf, kd, kw, rest = run_and_check(c, mask, tag, split_check=True)
             k = kf | kd | kw
             assert launched(k, lambda k: FIXUP_FWD | FIXUP_WGRAD <= k, rest[-1]) == fix, (tag, fix, sorted(k))
