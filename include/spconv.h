@@ -44,8 +44,15 @@ enum { SPC_POOL_MAX = 0, SPC_POOL_AVG = 1 };
  * Error bound per element, with A = the same operation on |x|, |w|, |dy| (and |b|) in exact arithmetic:
  *   inputs already tf32-representable:  |got - exact| <= 2^-12 A
  *   arbitrary fp32 inputs:              |got - exact| <= (2^-9 + 2^-12) A
+ * SPC_ALGO_TF32_ALL: SPC_ALGO_TF32, plus fprop, dgrad and wgrad of the fp32 stride-1 multi-tap filters: odd R x S up to
+ * 7 x 7 (3x3, 1x7, 7x1, ...), "same" padding, any N, C, K, H, and W % 4 == 0.  Their 1x1 layers run exactly as with
+ * SPC_ALGO_TF32 (same kernels, bit-identical results); every other fp32 shape runs on the direct kernels, and bf16 as
+ * with AUTO.  Rounding (fprop / dgrad: both operands to nearest tf32; wgrad: x to nearest, dy truncated) and error
+ * bound are those of SPC_ALGO_TF32 above, with A summed over all taps.  With halo strips the interior runs on the
+ * tensor cores with zero padding; the forward's outputs whose windows reach a strip are recomputed, and wgrad's share
+ * of the strips is added, in fp32 on the direct kernel.
  * SPC_ALGO_TCGEN05 still rejects fp32 (SPC_EUNSUPPORTED). */
-enum { SPC_ALGO_AUTO = 0, SPC_ALGO_DIRECT = 1, SPC_ALGO_TCGEN05 = 2, SPC_ALGO_TF32 = 3 };
+enum { SPC_ALGO_AUTO = 0, SPC_ALGO_DIRECT = 1, SPC_ALGO_TCGEN05 = 2, SPC_ALGO_TF32 = 3, SPC_ALGO_TF32_ALL = 4 };
 
 /* Geometry of one spatially-partitioned convolution on one tile.
  * Mirrors conv_spatial.__init__ (spatial.py:26-155): padding is "same"

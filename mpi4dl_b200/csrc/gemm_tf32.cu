@@ -22,30 +22,15 @@ namespace spc {
 
 int tc_sm_count();
 
-namespace {
-
-using namespace tc;
-
-constexpr int T_THREADS = 384;
-constexpr int T_BK = 32;                      // channels (fprop) / pixels (wgrad) per stage: one 128-byte fp32 row
-constexpr int T_BN = 128;                     // pixels per fprop tile: four 32-pixel boxes
-constexpr int T_XBOX = 32 * T_BK * 4;         // one [32 ch][32 px] box: 4 KB
-constexpr int T_XSTAGE = 4 * T_XBOX;          // a tile's [32 ch][128 px]: 16 KB
-constexpr int T_OUT_CH = 64;                  // output channels per epilogue staging block
-constexpr int T_OUT_BYTES = T_OUT_CH * T_BN * 4;   // 32 KB: [4 px boxes][64 ch][128 B]
-constexpr int T_MAX_STAGES = 8;
-constexpr int T_SMEM_LIMIT = 222 * 1024;      // as gemm_tc.cu: room for a small co-resident kernel
-constexpr int T_SMEM_AUX = 1024 /*align*/ + 512 /*barriers*/;
-constexpr int T_A_BLK = 128 * 128;            // wgrad: one 128-row block of dY, 32 pixels: 16 KB
-
 // ---- host: fp32 TMA descriptors ----------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-// fp32 tensor map with SWIZZLE_128B, rank 2 or 3; dims innermost first, strides in bytes (dims 1..)
+// fp32 tensor map with SWIZZLE_128B (swizzle = false: none), rank 2 to 4 (conv_tap_tf32.cu uses it too); dims
+// innermost first, strides in bytes (dims 1..)
 int make_tmap_f32(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                  const uint32_t* box) {
+                  const uint32_t* box, bool swizzle) {
   static EncodeTiledFn enc = nullptr;
   if (!enc) {
     void* fp = nullptr;
@@ -66,8 +51,8 @@ int make_tmap_f32(CUtensorMap* m, const void* base, int rank, const uint64_t* di
     }
     ctx_bound = true;
   }
-  cuuint64_t gd[3], gs[2];
-  cuuint32_t bx[3], es[3];
+  cuuint64_t gd[4], gs[3];
+  cuuint32_t bx[4], es[4];
   for (int i = 0; i < rank; ++i) {
     gd[i] = dims[i];
     bx[i] = box[i];
@@ -75,7 +60,8 @@ int make_tmap_f32(CUtensorMap* m, const void* base, int rank, const uint64_t* di
     if (i > 0) gs[i - 1] = strides_bytes[i];
   }
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled (fp32) failed (%d) rank=%d dims=[%llu,%llu,%llu]", (int)r, rank,
@@ -85,12 +71,28 @@ int make_tmap_f32(CUtensorMap* m, const void* base, int rank, const uint64_t* di
   return SPC_OK;
 }
 
+namespace {
+
+using namespace tc;
+
+constexpr int T_THREADS = 384;
+constexpr int T_BK = 32;                      // channels (fprop) / pixels (wgrad) per stage: one 128-byte fp32 row
+constexpr int T_BN = 128;                     // pixels per fprop tile: four 32-pixel boxes
+constexpr int T_XBOX = 32 * T_BK * 4;         // one [32 ch][32 px] box: 4 KB
+constexpr int T_XSTAGE = 4 * T_XBOX;          // a tile's [32 ch][128 px]: 16 KB
+constexpr int T_OUT_CH = 64;                  // output channels per epilogue staging block
+constexpr int T_OUT_BYTES = T_OUT_CH * T_BN * 4;   // 32 KB: [4 px boxes][64 ch][128 B]
+constexpr int T_MAX_STAGES = 8;
+constexpr int T_SMEM_LIMIT = 222 * 1024;      // as gemm_tc.cu: room for a small co-resident kernel
+constexpr int T_SMEM_AUX = 1024 /*align*/ + 512 /*barriers*/;
+constexpr int T_A_BLK = 128 * 128;            // wgrad: one 128-row block of dY, 32 pixels: 16 KB
+
 // [N][rows][P] fp32 activations, box = [box_rows][32 px]
 int make_act_tmap_f32(CUtensorMap* m, const void* base, int P, int rows, int N, int box_rows) {
   const uint64_t dims[3] = {(uint64_t)P, (uint64_t)rows, (uint64_t)N};
   const uint64_t strides[3] = {0, (uint64_t)P * 4, (uint64_t)P * rows * 4};
   const uint32_t box[3] = {32, (uint32_t)box_rows, 1};
-  return make_tmap_f32(m, base, 3, dims, strides, box);
+  return make_tmap_f32(m, base, 3, dims, strides, box, true);
 }
 
 inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
@@ -339,7 +341,7 @@ int run_tf32_pw(const float* w, int transpose, int M, int Cin, const float* x, c
     const uint64_t dims[2] = {(uint64_t)Cpad, (uint64_t)Mpad};
     const uint64_t strides[2] = {0, (uint64_t)Cpad * 4};
     const uint32_t box[2] = {T_BK, (uint32_t)NT};
-    int rc = make_tmap_f32(&tw, wp, 2, dims, strides, box);
+    int rc = make_tmap_f32(&tw, wp, 2, dims, strides, box, true);
     if (rc) return rc;
   }
   int rc = make_act_tmap_f32(&tx, x, P, Cin, N, T_BK);

@@ -54,8 +54,12 @@ def _ptr(t):
 
 def conv_algo_default():
     """Initial value of a conv layer's `algo`: SPCONV_ALLOW_TF32=1 lets the fp32 1x1 convolutions run on the TF32
-    tensor cores (SPC_ALGO_TF32: 10-bit mantissa products, fp32 sums; bf16 is unaffected), else SPC_ALGO_AUTO."""
-    return _lib.SPC_ALGO_TF32 if os.environ.get("SPCONV_ALLOW_TF32", "0") == "1" else _lib.SPC_ALGO_AUTO
+    tensor cores (SPC_ALGO_TF32: 10-bit mantissa products, fp32 sums; bf16 is unaffected), SPCONV_ALLOW_TF32=all
+    the stride-1 multi-tap ones too (SPC_ALGO_TF32_ALL), else SPC_ALGO_AUTO."""
+    v = os.environ.get("SPCONV_ALLOW_TF32", "0")
+    if v == "1":
+        return _lib.SPC_ALGO_TF32
+    return _lib.SPC_ALGO_TF32_ALL if v == "all" else _lib.SPC_ALGO_AUTO
 
 
 class _SpatialTopology:
