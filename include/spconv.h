@@ -51,8 +51,16 @@ enum { SPC_POOL_MAX = 0, SPC_POOL_AVG = 1 };
  * bound are those of SPC_ALGO_TF32 above, with A summed over all taps.  With halo strips the interior runs on the
  * tensor cores with zero padding; the forward's outputs whose windows reach a strip are recomputed, and wgrad's share
  * of the strips is added, in fp32 on the direct kernel.
+ * SPC_ALGO_TF32_STRIDED: SPC_ALGO_TF32_ALL (same kernels, bit-identical results on the shapes it takes), plus fprop,
+ * dgrad and wgrad of the fp32 multi-tap filters with stride_h == stride_w == 2: R and S each 3, 5 or 7, "same" padding,
+ * even H, W % 8 == 0, any N, C, K.  dgrad writes all of dx.  1x7 / 7x1 at stride 2, mixed strides and every other fp32
+ * shape run on the direct kernels.  Rounding, error bound and the treatment of halo strips are those of
+ * SPC_ALGO_TF32_ALL above (dgrad has no halo).
  * SPC_ALGO_TCGEN05 still rejects fp32 (SPC_EUNSUPPORTED). */
-enum { SPC_ALGO_AUTO = 0, SPC_ALGO_DIRECT = 1, SPC_ALGO_TCGEN05 = 2, SPC_ALGO_TF32 = 3, SPC_ALGO_TF32_ALL = 4 };
+enum {
+  SPC_ALGO_AUTO = 0, SPC_ALGO_DIRECT = 1, SPC_ALGO_TCGEN05 = 2, SPC_ALGO_TF32 = 3, SPC_ALGO_TF32_ALL = 4,
+  SPC_ALGO_TF32_STRIDED = 5
+};
 
 /* Geometry of one spatially-partitioned convolution on one tile.
  * Mirrors conv_spatial.__init__ (spatial.py:26-155): padding is "same"

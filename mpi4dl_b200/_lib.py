@@ -8,7 +8,7 @@ LIB_PATH = os.path.join(HERE, "libspconv.so")
 
 SPC_F32, SPC_BF16 = 0, 1
 SPC_POOL_MAX, SPC_POOL_AVG = 0, 1
-SPC_ALGO_AUTO, SPC_ALGO_DIRECT, SPC_ALGO_TCGEN05, SPC_ALGO_TF32, SPC_ALGO_TF32_ALL = 0, 1, 2, 3, 4
+SPC_ALGO_AUTO, SPC_ALGO_DIRECT, SPC_ALGO_TCGEN05, SPC_ALGO_TF32, SPC_ALGO_TF32_ALL, SPC_ALGO_TF32_STRIDED = 0, 1, 2, 3, 4, 5
 IPC_HANDLE_BYTES = 64
 
 

@@ -7,7 +7,8 @@
 // the halo exchange -- the overlap the reference left as dead code (spatial.py:415-866).
 // fp32 runs there only when the caller opts in: SPC_ALGO_TF32 for its 1x1 layers (gemm_tf32.cu, which have no halo),
 // SPC_ALGO_TF32_ALL for those and the stride-1 multi-tap layers (conv_tap_tf32.cu: the interior with zero padding; the
-// forward's boundary strips are recomputed on the direct kernel, and wgrad adds the strips' share on it).
+// forward's boundary strips are recomputed on the direct kernel, and wgrad adds the strips' share on it),
+// SPC_ALGO_TF32_STRIDED for all of those and the stride-2 multi-tap layers (conv_tap_s2_tf32.cu, the same plan).
 // Everything else runs entirely on the direct kernel; when its interior and boundary passes are
 // split (spc_conv2d_fwd_interior / _boundary, fp32 or SPC_ALGO_DIRECT), it recomputes the strips.
 #include "common.cuh"
@@ -155,21 +156,25 @@ int spc_conv_uses_tcgen05(const spc_conv_desc* d, int op) {
   if (!d || d->algo == SPC_ALGO_DIRECT) return 0;
   // fp32 storage reaches the tensor cores only when the caller opts in to TF32 (gemm_tf32.cu, conv_tap_tf32.cu)
   if (d->dtype == SPC_F32) {
-    if (d->algo != SPC_ALGO_TF32 && d->algo != SPC_ALGO_TF32_ALL) return 0;
+    if (d->algo != SPC_ALGO_TF32 && d->algo != SPC_ALGO_TF32_ALL && d->algo != SPC_ALGO_TF32_STRIDED) return 0;
     if (tf32_supported(d)) return 1;
-    return (d->algo == SPC_ALGO_TF32_ALL && tf32_tap_supported(d)) ? 1 : 0;
+    if (d->algo != SPC_ALGO_TF32 && tf32_tap_supported(d)) return 1;
+    return (d->algo == SPC_ALGO_TF32_STRIDED && tf32_tap_s2_supported(d)) ? 1 : 0;
   }
   return tc_supported(d, op) ? 1 : 0;
 }
 
-// fp32 on the tensor cores: the 1x1 GEMM (gemm_tf32.cu) or the tap kernels (conv_tap_tf32.cu)
+// fp32 on the tensor cores: the 1x1 GEMM (gemm_tf32.cu) or the tap kernels of stride 1 (conv_tap_tf32.cu) / stride 2
+// (conv_tap_s2_tf32.cu)
 static bool tf32_pointwise(const spc_conv_desc* d) { return d->R == 1 && d->S == 1; }
+static bool tf32_strided(const spc_conv_desc* d) { return d->stride_h == 2; }
 
 size_t spc_conv_workspace_bytes(const spc_conv_desc* d, int op) {
   if (!d) return 0;
   if (!spc_conv_uses_tcgen05(d, op)) return 0;
   if (d->dtype == SPC_BF16) return tc_workspace_bytes(d, op);
-  return tf32_pointwise(d) ? tf32_workspace_bytes(d, op) : tf32_tap_workspace_bytes(d, op);
+  if (tf32_pointwise(d)) return tf32_workspace_bytes(d, op);
+  return tf32_strided(d) ? tf32_tap_s2_workspace_bytes(d, op) : tf32_tap_workspace_bytes(d, op);
 }
 
 // Boundary strips: output rows / columns whose window reaches outside the tile, recomputed from
@@ -194,9 +199,11 @@ static int fwd_interior(const spc_conv_desc* d, const void* x, const void* w, co
     set_error("conv_fwd: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
     return SPC_EUNSUPPORTED;
   }
-  if (tc && d->dtype == SPC_F32)
-    return tf32_pointwise(d) ? tf32_conv_fwd(d, x, w, bias, y, workspace, workspace_bytes, st)
-                             : tf32_tap_fwd(d, x, w, bias, y, workspace, workspace_bytes, st);
+  if (tc && d->dtype == SPC_F32) {
+    if (tf32_pointwise(d)) return tf32_conv_fwd(d, x, w, bias, y, workspace, workspace_bytes, st);
+    return tf32_strided(d) ? tf32_tap_s2_fwd(d, x, w, bias, y, workspace, workspace_bytes, st)
+                           : tf32_tap_fwd(d, x, w, bias, y, workspace, workspace_bytes, st);
+  }
   if (tc) return tc_conv_fwd(d, x, w, bias, y, workspace, workspace_bytes, st);
   return launch_conv_direct(fwd_params(d, x, nullptr, w, bias, y), d->dtype, st);
 }
@@ -245,9 +252,11 @@ int spc_conv2d_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void
     set_error("conv_dgrad: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
     return SPC_EUNSUPPORTED;
   }
-  if (tc && d->dtype == SPC_F32)
-    return tf32_pointwise(d) ? tf32_conv_dgrad(d, dy, w, dx, workspace, workspace_bytes, st)
-                             : tf32_tap_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
+  if (tc && d->dtype == SPC_F32) {
+    if (tf32_pointwise(d)) return tf32_conv_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
+    return tf32_strided(d) ? tf32_tap_s2_dgrad(d, dy, w, dx, workspace, workspace_bytes, st)
+                           : tf32_tap_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
+  }
   if (tc) return tc_conv_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
 
   int Ho, Wo;
@@ -313,7 +322,7 @@ int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo
     rc = tf32_conv_wgrad(d, x, dy, dw, workspace, workspace_bytes, st);
     if (rc) return rc;
   } else if (tc && d->dtype == SPC_F32) {
-    rc = tf32_tap_wgrad(d, x, dy, dw, st);
+    rc = tf32_strided(d) ? tf32_tap_s2_wgrad(d, x, dy, dw, st) : tf32_tap_wgrad(d, x, dy, dw, st);
     if (rc) return rc;
     // the halo pixels' share (exact by linearity): the direct kernel over the outputs whose windows reach a strip,
     // reading the strips through the halo-only view (zero inside the tile)
@@ -323,7 +332,7 @@ int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo
         DirectWgradParams q{};
         q.in = make_view(nullptr, halo, d->N, d->C, d->H, d->W, d->pad_h, d->pad_w);
         q.dy = dy; q.dw = dw;
-        q.K = d->K; q.R = d->R; q.S = d->S; q.sh = 1; q.sw = 1; q.ph = d->pad_h; q.pw = d->pad_w;
+        q.K = d->K; q.R = d->R; q.S = d->S; q.sh = d->stride_h; q.sw = d->stride_w; q.ph = d->pad_h; q.pw = d->pad_w;
         q.Ho = Ho; q.Wo = Wo;
         q.ry0 = b.y0[i]; q.rx0 = b.x0[i]; q.rH = b.y1[i] - b.y0[i]; q.rW = b.x1[i] - b.x0[i];
         rc = launch_wgrad_direct(q, SPC_F32, st);

@@ -197,4 +197,14 @@ int tf32_tap_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* 
 // the interior's share of dw (zero padding), added with atomics; api.cu adds the halo strips' share
 int tf32_tap_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st);
 
+// ---- fp32 stride-2 multi-tap convolutions on TF32 wgmma (SPC_ALGO_TF32_STRIDED): conv_tap_s2_tf32.cu ---------------
+bool tf32_tap_s2_supported(const spc_conv_desc* d);
+size_t tf32_tap_s2_workspace_bytes(const spc_conv_desc* d, int op);
+int tf32_tap_s2_fwd(const spc_conv_desc* d, const void* x, const void* w, const void* bias, void* y, void* ws,
+                    size_t ws_bytes, cudaStream_t st);
+int tf32_tap_s2_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* dx, void* ws, size_t ws_bytes,
+                      cudaStream_t st);
+// the interior's share of dw (zero padding), added with atomics; api.cu adds the halo strips' share
+int tf32_tap_s2_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st);
+
 }  // namespace spc

@@ -25,51 +25,20 @@
 // tf32-representable inputs (exact products) the result meets include/spconv.h's 2^-12 A, and with arbitrary inputs the
 // rounding of both operands to tf32 (2^-11 relative each) adds the rest of (2^-9 + 2^-12) A.
 // Warp roles (384 threads): warp 0 = TMA producer, warpgroups 1 and 2 = wgmma consumers.  Persistent CTAs.
-#include "common.cuh"
-#include "tc_common.cuh"
-#include "wgmma_tf32.cuh"
+#include "tap_tf32_common.cuh"
 
 namespace spc {
-
-int tc_sm_count();
-int make_tmap_f32(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                  const uint32_t* box, bool swizzle);   // gemm_tf32.cu
 
 namespace {
 
 using namespace tc;
 
-constexpr int TT_THREADS = 384;
-constexpr int TT_BK = 32;                     // channels per k-chunk / pixels per row segment
 constexpr int TT_XW = 40;                     // pixels per box row: a segment and 4 pixels of slack on each side
 constexpr int TT_SEG = TT_BK * TT_XW * 4;     // one [32 ch][40 px] box: 5 KB
 constexpr int TT_XSTAGE = 4 * TT_SEG;         // a tile's four segments: 20 KB
-constexpr int TT_MAX_STAGES = 8;
-constexpr int TT_SMEM_LIMIT = 222 * 1024;     // as gemm_tf32.cu
-constexpr int TT_SMEM_AUX = 1024 /*align*/ + 512 /*barriers*/;
-constexpr int TT_WRES_MAX = 128 * 1024;       // resident weights at most
 constexpr int TT_SMALL_SEG = 8 * TT_XW * 4;   // small-Cin mode: one [8 ch][40 px] box: 1280 B
 constexpr int TW_XW = 44;                     // wgrad: pixels per box row (4 slack left, 8 right; pitch 12 mod 32)
 constexpr int TW_XBOX = 128 * TW_XW * 4;      // wgrad: one [128 ch][44 px] box: 22 KB
-constexpr int TW_MAX_CHAIN = 512;             // wgrad: row segments per item at most (the error bound above)
-
-inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
-inline size_t align1k(size_t b) { return (b + 1023) & ~(size_t)1023; }
-
-__device__ __forceinline__ uint32_t to_tf32(float v) {   // round to nearest, ties away (the low 13 bits become 0)
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-  return r;
-}
-
-// [N][rows][H][W] fp32, box = [1][box_rows][1][box_w px]
-int make_act_tmap4(CUtensorMap* m, const void* base, int N, int rows, int H, int W, int box_rows, int box_w,
-                   bool swizzle) {
-  const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)rows, (uint64_t)N};
-  const uint64_t strides[4] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4, (uint64_t)rows * H * W * 4};
-  const uint32_t box[4] = {(uint32_t)box_w, 1, (uint32_t)box_rows, 1};
-  return make_tmap_f32(m, base, 4, dims, strides, box, swizzle);
-}
 
 // ---- weight repack: Wp[rb][m][pos] = tf32(filter value), zero padded to [blocks][Mpad][Cpad] ------------------------
 //   fprop: m = k, c = input channel, w[m][c][r][s]      dgrad: m = input channel, c = k, w[c][m][R-1-r][S-1-s]
@@ -108,13 +77,6 @@ struct TapParams {
   int stages, wres, out_bufs;
   const float* bias;     // [M] or null
 };
-
-__device__ __forceinline__ void seg_coords(int seg, int segs_row, int H, int& n, int& y, int& x0) {
-  x0 = (seg % segs_row) * 32;
-  const int row = seg / segs_row;
-  y = row % H;
-  n = row / H;
-}
 
 // SMALL: the small-Cin mode (a template parameter, so that the general path compiles as if it did not exist)
 template <int NT, int SMALL>
@@ -287,9 +249,6 @@ tf32_tap_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_co
     if (leader) tma_store_wait_read<0>();
   }
 }
-
-// output channels per group: one wgmma N of 16, 32, 64, 128 or 256
-inline int tap_nt(int M) { return M <= 16 ? 16 : (M <= 32 ? 32 : (M <= 64 ? 64 : (M <= 128 ? 128 : 256))); }
 
 template <int NT, int SMALL>
 int launch_tap_gemm(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& ty, TapParams p, cudaStream_t st) {

@@ -55,11 +55,11 @@ def _ptr(t):
 def conv_algo_default():
     """Initial value of a conv layer's `algo`: SPCONV_ALLOW_TF32=1 lets the fp32 1x1 convolutions run on the TF32
     tensor cores (SPC_ALGO_TF32: 10-bit mantissa products, fp32 sums; bf16 is unaffected), SPCONV_ALLOW_TF32=all
-    the stride-1 multi-tap ones too (SPC_ALGO_TF32_ALL), else SPC_ALGO_AUTO."""
+    the stride-1 multi-tap ones too (SPC_ALGO_TF32_ALL), SPCONV_ALLOW_TF32=strided also the stride-2 3x3 / 5x5 / 7x7
+    ones (SPC_ALGO_TF32_STRIDED), else SPC_ALGO_AUTO."""
     v = os.environ.get("SPCONV_ALLOW_TF32", "0")
-    if v == "1":
-        return _lib.SPC_ALGO_TF32
-    return _lib.SPC_ALGO_TF32_ALL if v == "all" else _lib.SPC_ALGO_AUTO
+    return {"1": _lib.SPC_ALGO_TF32, "all": _lib.SPC_ALGO_TF32_ALL,
+            "strided": _lib.SPC_ALGO_TF32_STRIDED}.get(v, _lib.SPC_ALGO_AUTO)
 
 
 class _SpatialTopology:
