@@ -25,7 +25,8 @@ from mpi4dl_b200.torchgems.mp_pipeline import model_generator  # noqa: E402
 
 def main(kind):
     p = parser.get_parser()
-    p.add_argument("--dtype", choices=["fp32", "bf16"], default="fp32")
+    p.add_argument("--dtype", choices=["fp32", "bf16", "bf16-amp"], default="fp32",
+                   help="bf16-amp: fp32 parameters, the forward under torch.autocast(dtype=torch.bfloat16)")
     p.add_argument("--steps", type=int, default=10)
     args = p.parse_args()
     gems_comm.initialize_cuda()
@@ -35,6 +36,7 @@ def main(kind):
     balance = [int(v) for v in args.balance.split(",")] if args.balance else None
     mb = int(batch_size / parts)
     dtype = torch.bfloat16 if args.dtype == "bf16" else torch.float32
+    amp_dtype = torch.bfloat16 if args.dtype == "bf16-amp" else None
 
     mpi_comm = gems_comm.MPIComm(split_size=mp_size, ENABLE_MASTER=True)
     local_rank = mpi_comm.rank % mp_size
@@ -51,7 +53,7 @@ def main(kind):
         g.ready_model(split_rank=stage)
         gens.append(g)
     tm_master = train_model_master(gens[0], gens[1], local_rank, batch_size, args.num_epochs, parts=parts, ASYNC=True,
-                                   replications=int(times / 2))
+                                   replications=int(times / 2), amp_dtype=amp_dtype)
     sync_allreduce = gems_comm.SyncAllreduce(mpi_comm)
     sync_allreduce.sync_model(gens[0], gens[1])
 

@@ -31,7 +31,8 @@ from mpi4dl_b200.torchgems.train_spatial_master import train_spatial_model_maste
 
 def main(kind):
     p = parser.get_parser()
-    p.add_argument("--dtype", choices=["fp32", "bf16"], default="fp32")
+    p.add_argument("--dtype", choices=["fp32", "bf16", "bf16-amp"], default="fp32",
+                   help="bf16-amp: fp32 parameters, the forward under torch.autocast(dtype=torch.bfloat16)")
     p.add_argument("--steps", type=int, default=10)
     args = p.parse_args()
     gems_comm.initialize_cuda()
@@ -49,6 +50,7 @@ def main(kind):
         raise NotImplementedError("--local-DP > 1 is not built")
     mb = int(batch_size / parts)
     dtype = torch.bfloat16 if args.dtype == "bf16" else torch.float32
+    amp_dtype = torch.bfloat16 if args.dtype == "bf16-amp" else None
 
     comm1 = gems_comm.MPIComm(split_size=split_size, ENABLE_MASTER=False, ENABLE_SPATIAL=True,
                               num_spatial_parts=num_spatial_parts, spatial_size=spatial_size, LOCAL_DP_LP=1)
@@ -75,7 +77,8 @@ def main(kind):
         g.ready_model(split_rank=comm.split_rank)
         gens.append(g)
     master = train_spatial_model_master(gens[0], gens[1], batch_size, spatial_size, num_spatial_parts, slice_method, comm1,
-                                        comm2, LOCAL_DP_LP=1, parts=parts, ASYNC=True, replications=int(times / 2))
+                                        comm2, LOCAL_DP_LP=1, parts=parts, ASYNC=True, replications=int(times / 2),
+                                        amp_dtype=amp_dtype)
     sync = gems_comm.SyncAllreduce(comm1)
     n_img = batch_size * 2 * int(times / 2)
 

@@ -23,7 +23,8 @@ from mpi4dl_b200.torchgems.mp_pipeline import model_generator, train_model  # no
 
 def main(kind):
     p = parser.get_parser()
-    p.add_argument("--dtype", choices=["fp32", "bf16"], default="fp32")
+    p.add_argument("--dtype", choices=["fp32", "bf16", "bf16-amp"], default="fp32",
+                   help="bf16-amp: fp32 parameters, the forward under torch.autocast(dtype=torch.bfloat16)")
     p.add_argument("--steps", type=int, default=10)
     args = p.parse_args()
     gems_comm.initialize_cuda()
@@ -32,6 +33,7 @@ def main(kind):
     balance = [int(v) for v in args.balance.split(",")] if args.balance else None
     mb = int(batch_size / parts)
     dtype = torch.bfloat16 if args.dtype == "bf16" else torch.float32
+    amp_dtype = torch.bfloat16 if args.dtype == "bf16-amp" else None
 
     mpi_comm = gems_comm.MPIComm(split_size=mp_size, ENABLE_MASTER=False)
     local_rank = mpi_comm.rank % mp_size
@@ -44,7 +46,7 @@ def main(kind):
     model_gen = model_generator(model=make_model().to(dtype), split_size=mp_size, input_size=(mb, 3, image_size, image_size),
                                 balance=balance, shape_list=shapes)
     model_gen.ready_model(split_rank=local_rank)
-    tm = train_model(model_gen, local_rank, batch_size, args.num_epochs, parts=parts, ASYNC=True)
+    tm = train_model(model_gen, local_rank, batch_size, args.num_epochs, parts=parts, ASYNC=True, amp_dtype=amp_dtype)
     sync_allreduce = gems_comm.SyncAllreduce(mpi_comm)
     replicas = mpi_comm.size // mp_size
 

@@ -9,8 +9,8 @@ Same command line as the reference's benchmarks/spatial_parallelism/benchmark_{r
         --slice-method square --split-size 2 --batch-size 1 --num-layers 18 --num-filters 416 --dtype bf16
 
 world size = spatial_size * P + split_size - spatial_size.  Extra flags of this script: --dtype
-{fp32,bf16} (bf16 puts the spatial convs on the wgmma kernels), --steps N (synthetic batches per
-epoch, default 10).  APP 3 (synthetic) needs no dataset; APP 1/2 use torchvision like the reference.
+{fp32,bf16,bf16-amp} (bf16 puts the spatial convs on the wgmma kernels; bf16-amp too, with fp32
+master weights under torch.autocast), --steps N (synthetic batches per epoch, default 10).  APP 3 (synthetic) needs no dataset; APP 1/2 use torchvision like the reference.
 """
 import math
 import os
@@ -85,7 +85,8 @@ def _batches(args, image_size, batch_size, steps):
 
 def main(kind):
     p = parser.get_parser()
-    p.add_argument("--dtype", choices=["fp32", "bf16"], default="fp32")
+    p.add_argument("--dtype", choices=["fp32", "bf16", "bf16-amp"], default="fp32",
+                   help="bf16-amp: fp32 parameters, the forward under torch.autocast(dtype=torch.bfloat16)")
     p.add_argument("--steps", type=int, default=10)
     args = p.parse_args()
     gems_comm.initialize_cuda()
@@ -107,6 +108,7 @@ def main(kind):
     local_rank, split_rank = mpi_comm.rank, mpi_comm.split_rank
     mb = int(batch_size / parts)
     dtype = torch.bfloat16 if args.dtype == "bf16" else torch.float32
+    amp_dtype = torch.bfloat16 if args.dtype == "bf16-amp" else None
 
     spatial_kw = dict(input_shape=(mb, 3, image_size, image_size), local_rank=local_rank % P, mp_size=split_size,
                       balance=balance, spatial_size=spatial_size, num_spatial_parts=num_spatial_parts, slice_method=slice_method)
@@ -124,7 +126,7 @@ def main(kind):
     del model
     trainer = train_model_spatial(model_gen, local_rank, batch_size, epochs=1, spatial_size=spatial_size,
                                   num_spatial_parts=num_spatial_parts, parts=parts, ASYNC=True, GEMS_INVERSE=False,
-                                  slice_method=slice_method, mpi_comm=mpi_comm)
+                                  slice_method=slice_method, mpi_comm=mpi_comm, amp_dtype=amp_dtype)
     sync_allreduce.sync_model_spatial(model_gen)
     is_tile = local_rank < spatial_size * P
     cuda = torch.cuda.is_available()

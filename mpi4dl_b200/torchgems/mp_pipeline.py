@@ -5,7 +5,7 @@ trainer builds on.  Mirrors the reference's public surface (src/torchgems/mp_pip
         .get_start_end_layer_index / .get_model / .ready_model / .DDP_model / .get_output_shapes
         .models  .shape_list
     train_model(model_gen, local_rank, batch_size, epochs, criterion=None, optimizer=None,
-                parts=1, ASYNC=True, GEMS_INVERSE=False)                           :171-538
+                parts=1, ASYNC=True, GEMS_INVERSE=False, *, amp_dtype=None)        :171-538
         .run_step(x, y) -> (loss, corrects)  .forward_pass  .backward_pass  .update
 
 Host-side orchestration only (no kernels): activations travel forward and their gradients
@@ -17,6 +17,7 @@ sent in a fixed order), and receive buffers are plain `torch.empty`.
 """
 from collections import OrderedDict
 
+import contextlib
 import os
 
 import torch
@@ -113,7 +114,9 @@ class model_generator:
 
 class train_model:
     def __init__(self, model_gen, local_rank, batch_size, epochs, criterion=None, optimizer=None, parts=1, ASYNC=True,
-                 GEMS_INVERSE=False):
+                 GEMS_INVERSE=False, *, amp_dtype=None):
+        """amp_dtype=torch.bfloat16: the forward of this stage runs under torch.autocast with fp32 parameters (fp32
+        master weights, gradients and optimizer); activations and their gradients travel in bf16."""
         self.models = model_gen.models
         self.shape_list = model_gen.shape_list
         self.input_size = model_gen.input_size
@@ -124,8 +127,10 @@ class train_model:
         self.GEMS_INVERSE = GEMS_INVERSE
         self.batch_size = batch_size
         self.device = _device()
-        # activations travel in the model's dtype (fp32 as in the reference; bf16 when the model was cast)
-        self.dtype = next((p.dtype for p in self.models.parameters() if p.is_floating_point()), torch.float32)
+        # activations travel in the model's dtype (fp32 as in the reference; bf16 when the model was cast), or in the
+        # autocast dtype
+        self.amp_dtype = amp_dtype
+        self.dtype = amp_dtype or next((p.dtype for p in self.models.parameters() if p.is_floating_point()), torch.float32)
         # subclasses (train_model_spatial) set these before calling us
         if not hasattr(self, "num_spatial_parts"):
             self.num_spatial_parts = 1
@@ -213,6 +218,8 @@ class train_model:
     receive_input_async = receive_input_sync
 
     def send_input_sync(self, y):
+        if self.amp_dtype is not None:      # an op autocast runs in fp32 may end the stage: match the receive buffers
+            y = [t.to(self.dtype) for t in self._as_list(y)]
         self._send(y, self.to_send_forward)
 
     send_input_async = send_input_sync
@@ -228,13 +235,19 @@ class train_model:
     send_grad_async = send_grad_sync
 
     # ---- one micro-batch ----------------------------------------------------------------------
+    def _autocast(self):
+        if self.amp_dtype is None:
+            return contextlib.nullcontext()
+        return torch.autocast(self.device.type, dtype=self.amp_dtype)
+
     def forward_pass(self, data_x, data_y, part_number=0):
         if self.split_rank == 0:
             input_x = data_x
         else:
             self.receive_input_async(part_number)
             input_x = self.input_x_list[part_number]
-        y = self.models(input_x)
+        with self._autocast():
+            y = self.models(input_x)
         if self.split_rank != self.split_size - 1:
             self.send_input_async(y)
             return y, None
@@ -261,7 +274,7 @@ class train_model:
         """GPipe-style fill/drain: all micro-batch forwards, then all backwards (:509-534)."""
         data_x = data_x.to(self.device, non_blocking=True)
         data_y = data_y.to(self.device, non_blocking=True)
-        if data_x.is_floating_point() and data_x.dtype != self.dtype:
+        if data_x.is_floating_point() and data_x.dtype != self.dtype and self.amp_dtype is None:
             data_x = data_x.to(self.dtype)
         per = int(self.batch_size / self.parts)
         outs, loss, corrects = [], 0, 0

@@ -18,6 +18,7 @@ libspconv.so loads.
 import ctypes as C
 import math
 import os
+import warnings
 
 import torch
 import torch.distributed as dist
@@ -50,6 +51,36 @@ def _workspace(nbytes, device):
 
 def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(None)
+
+
+_fp16_autocast_warned = False
+
+
+def _bf16_autocast():
+    return torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16
+
+
+def _autocast_input(x):
+    """The conv layers under torch.autocast, the way nn.Conv2d behaves there.  bf16 autocast: the input is cast to
+    bf16 here (differentiably, so its gradient returns in the input's dtype) and the parameters inside
+    _ConvSpatialFn, so the bf16 kernels run while the parameters and their gradients stay in their own dtype.  fp16
+    autocast: libspconv has no fp16 kernels, so the input keeps its dtype, with one warning per process."""
+    if not torch.is_autocast_enabled("cuda"):
+        return x
+    if _bf16_autocast():
+        return x.to(torch.bfloat16)
+    global _fp16_autocast_warned
+    if not _fp16_autocast_warned:
+        _fp16_autocast_warned = True
+        warnings.warn("torch.autocast(dtype=torch.float16) is not supported by libspconv: conv_spatial and local_conv2d "
+                      "run in their input's dtype (use dtype=torch.bfloat16)", stacklevel=3)
+    return x
+
+
+def _check_dtypes(x, weight, who):
+    """Outside bf16 autocast the input and the parameters must have one dtype."""
+    if x.dtype != weight.dtype and not (x.dtype == torch.bfloat16 and _bf16_autocast()):
+        raise RuntimeError("%s: input dtype %s != weight dtype %s" % (who, x.dtype, weight.dtype))
 
 
 def conv_algo_default():
@@ -233,7 +264,11 @@ class _ConvSpatialFn(torch.autograd.Function):
     """fprop / dgrad / wgrad through the C ABI.  By default halo strips enter as constants: the
     reference unpacks them with in-place slice assignment of detached tensors, so no gradient ever
     flows back to a neighbour (SURVEY 8a N2).  Given the layer (exact backward), the gradient of
-    the received strips is sent back and added into the neighbours' dx."""
+    the received strips is sent back and added into the neighbours' dx.
+
+    Parameters of another dtype than x (fp32 master weights under bf16 autocast) are rounded to x's dtype HERE, and
+    the weight gradient is returned as the fp32 sum the wgrad kernel wrote: a cast before the Function would make
+    autograd round dW to bf16 on its way back to the fp32 parameter."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, desc_args, *strips):
@@ -248,6 +283,10 @@ class _ConvSpatialFn(torch.autograd.Function):
         ready = strips[9] if len(strips) > 9 else None
         ctx.layer = strips[10] if len(strips) > 10 else None
         strips = strips[:9]
+        ctx.param_dtype = weight.dtype
+        if weight.dtype != x.dtype:           # round to nearest even; dgrad and the strip gradients use the same copy
+            weight = weight.to(x.dtype)
+            bias = bias.to(x.dtype) if bias is not None else None
         Ho, Wo = C.c_int(), C.c_int()
         L.spc_conv_out_shape(C.byref(d), C.byref(Ho), C.byref(Wo))
         y = torch.empty((d.N, d.K, Ho.value, Wo.value), dtype=x.dtype, device=x.device)
@@ -298,8 +337,8 @@ class _ConvSpatialFn(torch.autograd.Function):
             ws, wsp = _workspace(L.spc_conv_workspace_bytes(C.byref(d), 2), x.device)
             _lib.check(L.spc_conv2d_wgrad(C.byref(d), _ptr(x), C.byref(halo), _ptr(gy), _ptr(dw32), _ptr(db32), 0,
                                           wsp, 0 if ws is None else ws.numel(), _stream()), "spc_conv2d_wgrad")
-            dw = dw32.to(weight.dtype)
-            db = db32.to(weight.dtype) if db32 is not None else None
+            dw = dw32.to(ctx.param_dtype)
+            db = db32.to(ctx.param_dtype) if db32 is not None else None
         if exact:
             _reverse_finish(recv, ready, dx, d.pad_h, d.pad_w)
         return (dx, dw, db, None) + (None,) * ctx.n_tail
@@ -391,9 +430,8 @@ class conv_spatial(nn.Conv2d, _SpatialTopology):
 
     def forward(self, tensor):
         _require_cuda(tensor, "conv_spatial")
-        x = tensor.contiguous()
-        if x.dtype != self.weight.dtype:
-            raise RuntimeError("conv_spatial: input dtype %s != weight dtype %s" % (x.dtype, self.weight.dtype))
+        x = _autocast_input(tensor).contiguous()
+        _check_dtypes(x, self.weight, "conv_spatial")
         hh, hw = self.halo_len_height, self.halo_len_width
         H0, W0 = x.shape[2], x.shape[3]
         et = el = 0
@@ -605,9 +643,8 @@ class local_conv2d(nn.Conv2d):
 
     def forward(self, tensor):
         _require_cuda(tensor, "local_conv2d")
-        x = tensor.contiguous()
-        if x.dtype != self.weight.dtype:
-            raise RuntimeError("local_conv2d: input dtype %s != weight dtype %s" % (x.dtype, self.weight.dtype))
+        x = _autocast_input(tensor).contiguous()
+        _check_dtypes(x, self.weight, "local_conv2d")
         N, Cc, H, W = x.shape
         ph, pw = self._same
         desc_args = (N, Cc, H, W, self.out_channels, self.kernel_size[0], self.kernel_size[1], self.stride[0],
