@@ -37,6 +37,10 @@ bool wgrad_tap_supported(int K, int C, int R, int S, int H, int W, int stride);
 int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, int K, int C, int N, int H, int W, int R, int S,
                   cudaStream_t st);
 
+// gemm_px.cu: pixel-major 1x1 GEMM (output channels as the wgmma N dimension, NT per tile)
+int run_pw_px(int NT, const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& ty, int M, int Cin, int N, int P,
+              int x5, int y5, const __nv_bfloat16* bias, int sms, cudaStream_t st);
+
 namespace {
 
 constexpr int TC_THREADS = 384;
@@ -425,7 +429,21 @@ struct TcConv {
   int H, W, N;                 // input image
   int stride;                  // 1 or 2 (both axes)
   const __nv_bfloat16* prepacked;   // if set: weights already in [taps][Mpad][Cpad] layout (1024-aligned)
+  int px;                      // 1x1 only: large problems may run on pw_px_gemm_kernel (gemm_px.cu)
 };
+
+// Output channels per tile of pw_px_gemm_kernel for a layer with M output channels, or 0 where its tiles would not fit
+// M clearly better than pw_gemm_kernel's, which computes 128-row blocks in groups of two (M <= 128: one block).  NT is
+// the smallest instantiated tile width (56, 104, 208) that holds M, else 208 in several groups.  The tiles must waste
+// fewer MMA rows than the 128-row blocks and hold at least 90 % valid channels: 52 -> 56, 104 -> 104, 208 k -> k groups
+// of 208; 16, 64, 128 and 256 channels stay on pw_gemm_kernel.
+int px_tile_channels(int M) {
+  const int nt = M <= 56 ? 56 : (M <= 104 ? 104 : 208);
+  const int pad = round_up(M, nt);
+  const int blocks = (M + 127) / 128;
+  const int old_rows = (blocks >= 2 ? round_up(blocks, 2) : 1) * 128;
+  return (pad < old_rows && 10 * M >= 9 * pad) ? nt : 0;
+}
 
 // Y[N][M][H*W] = sum_taps Wp[tap][M x Cin] * shift_tap(X[N][Cin][H][W])  (+bias)
 int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bias, __nv_bfloat16* y, void* ws,
@@ -434,7 +452,11 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
   const int cs = c.stride;
   const int Ho = c.H / cs, Wo = c.W / cs;
   const int Pin = c.H * c.W, P = Ho * Wo;            // P: output pixels per image
-  const int Mpad = round_up(c.M, 128), Cpad = round_up(c.Cin, BK);
+  // pixel-major kernel: 1x1 layers whose output channels it tiles better, with at least two 128-pixel tiles per SM
+  // (below that the persistent CTAs get one tile each and pw_gemm_kernel's 128-row blocks cost no more)
+  const int nt = (c.px && taps == 1) ? px_tile_channels(c.M) : 0;
+  const bool px = nt && (long long)c.N * ((P + BN - 1) / BN) >= 2ll * sm_count();
+  const int Mpad = round_up(c.M, px ? nt : 128), Cpad = round_up(c.Cin, BK);
   const bool v2 = taps > 1 && !env_get("SPC_TAP_V1") && tap_v2_supported(c.M, c.Cin, c.R, c.S, c.H, c.W, c.N, cs);
   const bool copies = (c.S > 1 || cs > 1) && taps > 1 && !v2;   // column-shifted (and subsampled) copies of the input
   const uintptr_t ws0 = reinterpret_cast<uintptr_t>(ws);
@@ -474,11 +496,18 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
   {
     const uint64_t dims[2] = {(uint64_t)Cpad, (uint64_t)taps * Mpad};
     const uint64_t strides[2] = {0, (uint64_t)Cpad * 2};
-    const uint32_t box[2] = {BK, 128};
+    const uint32_t box[2] = {BK, px ? (uint32_t)nt : 128u};
     int rc = make_tmap(&tw, wp, 2, dims, strides, box);
     if (rc) return rc;
   }
   int rc;
+  if (px) {
+    rc = x5 ? make_act_tmap5(&tx, x, Pin, c.Cin, c.N, BK / 8, BN / 64) : make_act_tmap(&tx, x, Pin, c.Cin, c.N, BK);
+    if (rc) return rc;
+    rc = y5 ? make_act_tmap5(&ty, y, P, c.M, c.N, nt / 8, 2) : make_act_tmap(&ty, y, P, c.M, c.N, nt);
+    if (rc) return rc;
+    return run_pw_px(nt, tw, tx, ty, c.M, c.Cin, c.N, P, x5, y5, bias, sm_count(), st);
+  }
   if (taps > 1) {
     // (copies of) the input as [img][Cin][H][Wo]; img = n + s*N for the copy of filter column s
     const uint64_t dims[4] = {(uint64_t)Wo, (uint64_t)c.H, (uint64_t)c.Cin, (uint64_t)c.N * (copies ? c.S : 1)};
@@ -514,10 +543,12 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
   return mb == 2 ? launch_pw<2>(tw, tx, tx4, ty, p, st) : launch_pw<1>(tw, tx, tx4, ty, p, st);
 }
 
-// pointwise helper (1x1): Y[N][M][P] = Wp[M x Cin] * X[N][Cin][P]
+// pointwise helper (1x1): Y[N][M][P] = Wp[M x Cin] * X[N][Cin][P]; px = 0 keeps it on pw_gemm_kernel
 int run_pw(const __nv_bfloat16* w, int ld, int transpose, int M, int Cin, const __nv_bfloat16* x,
-           const __nv_bfloat16* bias, __nv_bfloat16* y, int N, int P, void* ws, size_t ws_bytes, cudaStream_t st) {
+           const __nv_bfloat16* bias, __nv_bfloat16* y, int N, int P, void* ws, size_t ws_bytes, cudaStream_t st,
+           int px = 1) {
   TcConv c{};
+  c.px = px;
   c.w = w;
   c.sm = transpose ? 1 : ld; c.sc = transpose ? ld : 1; c.flip = 0;
   c.M = M; c.Cin = Cin; c.R = 1; c.S = 1; c.ph = 0; c.pw = 0; c.H = 1; c.W = P; c.N = N; c.stride = 1;
@@ -1285,7 +1316,8 @@ size_t tc_pw_workspace_bytes(int M, int Cin) { return (size_t)round_up(M, 128) *
 int tc_pw_fwd(const void* w, int ld, int M, int Cin, const void* x, const void* bias, void* y, int P, void* ws, size_t ws_bytes,
               cudaStream_t st) {
   return run_pw(reinterpret_cast<const __nv_bfloat16*>(w), ld, 0, M, Cin, reinterpret_cast<const __nv_bfloat16*>(x),
-                reinterpret_cast<const __nv_bfloat16*>(bias), reinterpret_cast<__nv_bfloat16*>(y), 1, P, ws, ws_bytes, st);
+                reinterpret_cast<const __nv_bfloat16*>(bias), reinterpret_cast<__nv_bfloat16*>(y), 1, P, ws, ws_bytes, st,
+                0);
 }
 int tc_pw_wgrad(const void* x, const void* dy, float* dw, int K, int C, int P, cudaStream_t st) {
   return run_wgrad(reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(dy), dw, K, C, 1, 1, P, 1, 1, 1,
