@@ -44,8 +44,11 @@ def build(arm):
     return m.to(torch.bfloat16) if arm == "bf16" else m
 
 
-def measure(arm, image, steps, warmup):
+def measure(arm, image, steps, warmup, recompute=False):
     m = build(arm)
+    if recompute:
+        from mpi4dl_b200.torchgems.recompute import checkpoint_spatial_cells
+        checkpoint_spatial_cells(m)
     opt = torch.optim.SGD(m.parameters(), lr=1e-3, momentum=0.9)
     x = torch.randn(1, 3, image, image, device="cuda", dtype=torch.bfloat16 if arm == "bf16" else torch.float32)
 

@@ -33,6 +33,8 @@ def main(kind):
     p = parser.get_parser()
     p.add_argument("--dtype", choices=["fp32", "bf16", "bf16-amp"], default="fp32",
                    help="bf16-amp: fp32 parameters, the forward under torch.autocast(dtype=torch.bfloat16)")
+    p.add_argument("--recompute", action="store_true",
+                   help="keep only each spatial cell's input and halo strips for backward and recompute the cell there")
     p.add_argument("--steps", type=int, default=10)
     args = p.parse_args()
     gems_comm.initialize_cuda()
@@ -78,7 +80,7 @@ def main(kind):
         gens.append(g)
     master = train_spatial_model_master(gens[0], gens[1], batch_size, spatial_size, num_spatial_parts, slice_method, comm1,
                                         comm2, LOCAL_DP_LP=1, parts=parts, ASYNC=True, replications=int(times / 2),
-                                        amp_dtype=amp_dtype)
+                                        amp_dtype=amp_dtype, recompute=args.recompute)
     sync = gems_comm.SyncAllreduce(comm1)
     n_img = batch_size * 2 * int(times / 2)
 

@@ -10,7 +10,8 @@ Same command line as the reference's benchmarks/spatial_parallelism/benchmark_{r
 
 world size = spatial_size * P + split_size - spatial_size.  Extra flags of this script: --dtype
 {fp32,bf16,bf16-amp} (bf16 puts the spatial convs on the wgmma kernels; bf16-amp too, with fp32
-master weights under torch.autocast), --steps N (synthetic batches per epoch, default 10).  APP 3 (synthetic) needs no dataset; APP 1/2 use torchvision like the reference.
+master weights under torch.autocast), --recompute (recompute the spatial cells in backward from their
+inputs and recorded halo strips), --steps N (synthetic batches per epoch, default 10).  APP 3 (synthetic) needs no dataset; APP 1/2 use torchvision like the reference.
 """
 import math
 import os
@@ -87,6 +88,8 @@ def main(kind):
     p = parser.get_parser()
     p.add_argument("--dtype", choices=["fp32", "bf16", "bf16-amp"], default="fp32",
                    help="bf16-amp: fp32 parameters, the forward under torch.autocast(dtype=torch.bfloat16)")
+    p.add_argument("--recompute", action="store_true",
+                   help="keep only each spatial cell's input and halo strips for backward and recompute the cell there")
     p.add_argument("--steps", type=int, default=10)
     args = p.parse_args()
     gems_comm.initialize_cuda()
@@ -126,7 +129,7 @@ def main(kind):
     del model
     trainer = train_model_spatial(model_gen, local_rank, batch_size, epochs=1, spatial_size=spatial_size,
                                   num_spatial_parts=num_spatial_parts, parts=parts, ASYNC=True, GEMS_INVERSE=False,
-                                  slice_method=slice_method, mpi_comm=mpi_comm, amp_dtype=amp_dtype)
+                                  slice_method=slice_method, mpi_comm=mpi_comm, amp_dtype=amp_dtype, recompute=args.recompute)
     sync_allreduce.sync_model_spatial(model_gen)
     is_tile = local_rank < spatial_size * P
     cuda = torch.cuda.is_available()

@@ -5,7 +5,8 @@ trainer builds on.  Mirrors the reference's public surface (src/torchgems/mp_pip
         .get_start_end_layer_index / .get_model / .ready_model / .DDP_model / .get_output_shapes
         .models  .shape_list
     train_model(model_gen, local_rank, batch_size, epochs, criterion=None, optimizer=None,
-                parts=1, ASYNC=True, GEMS_INVERSE=False, *, amp_dtype=None)        :171-538
+                parts=1, ASYNC=True, GEMS_INVERSE=False, *, amp_dtype=None,
+                recompute=False)                                                  :171-538
         .run_step(x, y) -> (loss, corrects)  .forward_pass  .backward_pass  .update
 
 Host-side orchestration only (no kernels): activations travel forward and their gradients
@@ -25,6 +26,8 @@ import torch.distributed as dist
 import torch.nn as nn
 import torch.optim as optim
 from torch.nn.parallel import DistributedDataParallel as DDP
+
+from .recompute import checkpoint_spatial_cells
 
 
 def _device():
@@ -114,10 +117,14 @@ class model_generator:
 
 class train_model:
     def __init__(self, model_gen, local_rank, batch_size, epochs, criterion=None, optimizer=None, parts=1, ASYNC=True,
-                 GEMS_INVERSE=False, *, amp_dtype=None):
+                 GEMS_INVERSE=False, *, amp_dtype=None, recompute=False):
         """amp_dtype=torch.bfloat16: the forward of this stage runs under torch.autocast with fp32 parameters (fp32
-        master weights, gradients and optimizer); activations and their gradients travel in bf16."""
+        master weights, gradients and optimizer); activations and their gradients travel in bf16.
+        recompute=True: the cells of this stage that contain a spatial layer keep only their inputs and received halo
+        strips for backward and run their forward again there (torchgems.recompute.checkpoint_spatial_cells)."""
         self.models = model_gen.models
+        if recompute:
+            checkpoint_spatial_cells(self.models)
         self.shape_list = model_gen.shape_list
         self.input_size = model_gen.input_size
         self.parts = parts

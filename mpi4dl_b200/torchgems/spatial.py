@@ -18,6 +18,7 @@ libspconv.so loads.
 import ctypes as C
 import math
 import os
+import threading
 import warnings
 
 import torch
@@ -91,6 +92,21 @@ def conv_algo_default():
     v = os.environ.get("SPCONV_ALLOW_TF32", "0")
     return {"1": _lib.SPC_ALGO_TF32, "all": _lib.SPC_ALGO_TF32_ALL,
             "strided": _lib.SPC_ALGO_TF32_STRIDED}.get(v, _lib.SPC_ALGO_AUTO)
+
+
+_recorder_state = threading.local()
+
+
+def _halo_recorder():
+    """The recorder of the recomputed region running on this thread (torchgems.recompute), or None."""
+    return getattr(_recorder_state, "rec", None)
+
+
+def _set_halo_recorder(rec):
+    """Make `rec` this thread's recorder; returns the previous one (to be restored by the caller)."""
+    prev = _halo_recorder()
+    _recorder_state.rec = rec
+    return prev
 
 
 class _SpatialTopology:
@@ -191,11 +207,20 @@ class _SpatialTopology:
     def _exchange(self, x, hh, hw):
         """Send the edge strips of `x` to the neighbours and return the 9 received strips
         (None where there is no neighbour).  Replaces start_halo_exchange / end_halo_exchange
-        (spatial.py:336-403)."""
+        (spatial.py:336-403).  Inside a recomputed region (torchgems.recompute) the forward appends the
+        received strips to the region's recorder, and the recompute in backward takes them back from it in the
+        same order without calling the transport."""
+        rec = _halo_recorder()
+        if rec is not None and rec.replaying:
+            return rec.replay(x, hh, hw)
         if self.neighbours is None or not any(self.neighbours):
-            return [None] * 9
-        tr = halo_transport.get_transport(x.device)
-        return tr.exchange(self, x, hh, hw, self.neighbours, self.rank_neighbours)
+            strips = [None] * 9
+        else:
+            tr = halo_transport.get_transport(x.device)
+            strips = tr.exchange(self, x, hh, hw, self.neighbours, self.rank_neighbours)
+        if rec is not None:
+            rec.record(strips)
+        return strips
 
 
 def _strip_shape(i, N, Cc, H, W, hh, hw):
@@ -443,7 +468,15 @@ class conv_spatial(nn.Conv2d, _SpatialTopology):
         exchange = (hh > 0 or hw > 0) and not self.fused_halo and self.neighbours is not None and any(self.neighbours)
         extra = ()
         with torch.no_grad():
-            if exchange and halo_transport.overlap_enabled():
+            rec = _halo_recorder()
+            if exchange and halo_transport.overlap_enabled() and rec is not None and rec.replaying:
+                # recompute: the replayed strips are complete, but the interior + boundary passes the forward ran are
+                # kept (spc_conv2d_fwd can differ from them in the last bit), so the recomputed y is the forward's
+                strips = self._exchange(x, hh, hw)
+                ready = torch.cuda.Event()
+                ready.record()
+                extra = (ready,)
+            elif exchange and halo_transport.overlap_enabled():
                 # exchange on the comm stream, overlapped with the interior pass on this stream
                 main = torch.cuda.current_stream()
                 comm = _comm_stream(x.device)
