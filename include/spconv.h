@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define SPC_VERSION 101
+#define SPC_VERSION 102
 
 enum { SPC_OK = 0, SPC_EINVAL = -1, SPC_ECUDA = -2, SPC_EUNSUPPORTED = -3, SPC_ENOMEM = -4 };
 enum { SPC_F32 = 0, SPC_BF16 = 1 };             /* storage dtype of x / w / y; accumulation is fp32 */
@@ -93,8 +93,6 @@ const char* spc_last_error(void);
 int         spc_device_info(int device, int* sm_count, int* cc);
 /* number of kernels this library has launched since the last reset (bench.py's gpu_launches) */
 long long   spc_launch_count(int reset);
-/* the SPC_* tuning knobs are read from the environment once per process; re-read them (dev probes only) */
-void        spc_reload_env(void);
 
 /* ---- convolution ------------------------------------------------------------------------ */
 /* y = conv(pad+halo(x), w) + bias.   Replaces spatial.py:1019-1029 (ZeroPad2d :1020,
@@ -206,28 +204,21 @@ int   spc_mailbox_export(spc_mailbox* mb, unsigned char handle[SPC_IPC_HANDLE_BY
 /* Map a peer's mailbox (handle obtained from the peer through torch.distributed). */
 int   spc_mailbox_open(spc_mailbox** out, const unsigned char handle[SPC_IPC_HANDLE_BYTES],
                        size_t bytes, int nflags);
-/* Fused protocol steps (one kernel each).  post: wait until local ack flags ack_idx[d] reach
- * ack_seq (0 = do not wait) -> pack every strip d with send[d] != NULL into send[d] (peer slot) ->
- * when the whole grid is done, publish `seq` on peers[d]'s arrival flag arrival_idx[d].
- * collect: wait for local arrival flags arrival_idx[d] >= seq -> copy bytes[d] from src[d] (local
- * mailbox slot) to dst[d] -> publish `seq` on peers[d]'s ack flag ack_idx[d]. */
-int spc_halo_post(int N, int C, int H, int W, int halo_h, int halo_w, int dtype, const void* x,
-                  void* const send[9], spc_mailbox* self, spc_mailbox* const peers[9],
-                  const int ack_idx[9], uint32_t ack_seq, const int arrival_idx[9], uint32_t seq,
-                  void* stream);
-int spc_halo_collect(void* const dst[9], const void* const src[9], const size_t bytes[9],
-                     spc_mailbox* self, spc_mailbox* const peers[9], const int arrival_idx[9],
-                     uint32_t seq, const int ack_idx[9], void* stream);
-/* Graph-capturable variants (what torchgems.halo_transport.PeerTransport uses): no host-side state in the
- * launch arguments.  The sequence number s of the exchange is (local flag seq_idx) + 1, read on the device;
- * its parity selects the half of the double-buffered slot (send0[d] / src0[d] + (s&1)*slot_bytes) and the
- * flag bank (index + (s&1)*9).  post waits for the acks of sequence s-2 (s <= 2: none); collect waits for
- * the arrivals of s, copies out, acks, and its last block stores s to flag seq_idx.  post and collect of one
- * exchange must be enqueued in that order on one stream.  counter_idx: a flag word private to the layer's
+/* Fused protocol steps (one kernel each), graph-capturable: no host-side state in the launch arguments.
+ *   post:    wait until the local ack flags ack_idx0[d] show that every neighbour has drained the slot half about
+ *            to be overwritten -> pack every strip d with send0[d] != NULL into send0[d] (peer slot) -> when the
+ *            whole grid is done, publish the sequence number on peers[d]'s arrival flag arrival_idx0[d].
+ *   collect: wait for the local arrival flags arrival_idx0[d] -> copy bytes[d] from src0[d] (local mailbox slot)
+ *            to dst[d] -> when the whole grid is done, publish the sequence number on peers[d]'s ack flag
+ *            ack_idx0[d] and store it to flag seq_idx.
+ * The sequence number s of the exchange is (local flag seq_idx) + 1, read on the device; its parity selects the
+ * half of the double-buffered slot (send0[d] / src0[d] + (s&1)*slot_bytes) and the flag bank (index + (s&1)*9).
+ * post waits for the acks of sequence s-2 (s <= 2: none); collect waits for the arrivals of s.  post and collect
+ * of one exchange must be enqueued in that order on one stream.  counter_idx: a flag word private to the layer's
  * slot, used as the grid-completion counter (exchanges of different layers may run on different streams).
  * The flag waits are bounded: after SPCONV_SPIN_TIMEOUT_S seconds (default 120, 0 = unbounded) the kernel
  * prints the direction it is stuck on and traps, so a dead peer surfaces as a CUDA error, not a hang.
- * Replaces the same reference lines as spc_halo_post / spc_halo_collect (spatial.py:336-403). */
+ * Replaces the reference's start_halo_exchange / end_halo_exchange (spatial.py:336-403). */
 int spc_halo_post_auto(int N, int C, int H, int W, int halo_h, int halo_w, int dtype, const void* x,
                        void* const send0[9], size_t slot_bytes, spc_mailbox* self,
                        spc_mailbox* const peers[9], const int ack_idx0[9], const int arrival_idx0[9],
@@ -267,10 +258,6 @@ int spc_halo_post_strips_auto(const void* const src[9], const size_t bytes[9], v
                               size_t slot_bytes, spc_mailbox* self, spc_mailbox* const peers[9],
                               const int ack_idx0[9], const int arrival_idx0[9], int seq_idx, int counter_idx,
                               void* stream);
-/* After writes to peer `mb` enqueued on `stream`: publish sequence number `seq` on flag `idx`. */
-int   spc_mailbox_signal(spc_mailbox* peer_mb, int idx, uint32_t seq, void* stream);
-/* Make `stream` wait (on device) until local flag `idx` reaches `seq`. */
-int   spc_mailbox_wait(spc_mailbox* mb, int idx, uint32_t seq, void* stream);
 
 #ifdef __cplusplus
 }

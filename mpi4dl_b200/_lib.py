@@ -32,7 +32,6 @@ SYMBOLS = [
     ("spc_last_error", C.c_char_p, []),
     ("spc_device_info", C.c_int, [C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     ("spc_launch_count", C.c_longlong, [C.c_int]),
-    ("spc_reload_env", None, []),
     ("spc_conv2d_fwd", C.c_int, [C.POINTER(ConvDesc), _P, C.POINTER(Halo), _P, _P, _P, _P, C.c_size_t, _P]),
     ("spc_conv2d_fwd_interior", C.c_int, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, C.c_size_t, _P]),
     ("spc_conv2d_fwd_boundary", C.c_int, [C.POINTER(ConvDesc), _P, C.POINTER(Halo), _P, _P, _P, _P]),
@@ -57,10 +56,6 @@ SYMBOLS = [
     ("spc_mailbox_data", _P, [_P]),
     ("spc_mailbox_export", C.c_int, [_P, C.c_char_p]),
     ("spc_mailbox_open", C.c_int, [C.POINTER(_P), C.c_char_p, C.c_size_t, C.c_int]),
-    ("spc_halo_post", C.c_int, [C.c_int] * 7 + [_P, C.POINTER(_P * 9), _P, C.POINTER(_P * 9), C.POINTER(C.c_int * 9),
-                                C.c_uint32, C.POINTER(C.c_int * 9), C.c_uint32, _P]),
-    ("spc_halo_collect", C.c_int, [C.POINTER(_P * 9), C.POINTER(_P * 9), C.POINTER(C.c_size_t * 9), _P, C.POINTER(_P * 9),
-                                   C.POINTER(C.c_int * 9), C.c_uint32, C.POINTER(C.c_int * 9), _P]),
     ("spc_halo_post_auto", C.c_int, [C.c_int] * 7 + [_P, C.POINTER(_P * 9), C.c_size_t, _P, C.POINTER(_P * 9),
                                      C.POINTER(C.c_int * 9), C.POINTER(C.c_int * 9), C.c_int, C.c_int, _P]),
     ("spc_halo_collect_auto", C.c_int, [C.POINTER(_P * 9), C.POINTER(_P * 9), C.POINTER(C.c_size_t * 9), C.c_size_t, _P,
@@ -73,8 +68,6 @@ SYMBOLS = [
     ("spc_halo_post_strips_auto", C.c_int, [C.POINTER(_P * 9), C.POINTER(C.c_size_t * 9), C.POINTER(_P * 9), C.c_size_t,
                                             _P, C.POINTER(_P * 9), C.POINTER(C.c_int * 9), C.POINTER(C.c_int * 9),
                                             C.c_int, C.c_int, _P]),
-    ("spc_mailbox_signal", C.c_int, [_P, C.c_int, C.c_uint32, _P]),
-    ("spc_mailbox_wait", C.c_int, [_P, C.c_int, C.c_uint32, _P]),
 ]
 
 _lib = None

@@ -340,7 +340,7 @@ int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo
       }
     }
   } else if (tc) {
-    rc = tc_conv_wgrad(d, x, dy, dw, /*accumulate=*/1, workspace, workspace_bytes, st);
+    rc = tc_conv_wgrad(d, x, dy, dw, workspace, workspace_bytes, st);
     if (rc) return rc;
     // add the halo pixels' contribution (exact by linearity): boundary GEMM over the outputs whose windows reach a strip
     if (has_halo(halo)) {

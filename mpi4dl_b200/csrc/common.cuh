@@ -174,8 +174,8 @@ int tc_conv_fwd(const spc_conv_desc* d, const void* x, const void* w, const void
                 void* ws, size_t ws_bytes, cudaStream_t st);
 int tc_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* dx, void* ws,
                   size_t ws_bytes, cudaStream_t st);
-int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, int accumulate,
-                  void* ws, size_t ws_bytes, cudaStream_t st);
+int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void* ws,
+                  size_t ws_bytes, cudaStream_t st);
 
 // ---- fp32 1x1 convolutions on TF32 wgmma (SPC_ALGO_TF32): gemm_tf32.cu ---------------------------------------------
 bool tf32_supported(const spc_conv_desc* d);

@@ -18,8 +18,6 @@
 //              [group][block][8 ch][128 B], which the GMMA descriptors express through LBO / SBO.
 // Warp roles (384 threads): warp 0 = TMA producer, warpgroups 1 and 2 = wgmma consumers + epilogue.
 // Persistent CTAs, one per SM.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -145,7 +143,6 @@ struct PwParams {
   int W, Mpad;                 // image width (tap mode: tiles are 64-pixel row segments), padded M
   int shiftN;                  // N when the activations are S column-shifted copies, else 0
   int rowmul;                  // input row = rowmul * output row + tap row offset (2 for stride-2 convs)
-  int tgroup;                  // consecutive tiles handled back-to-back by one CTA (DRAM page locality)
   const __nv_bfloat16* bias;   // [M] or null
   int x5, y5;                  // 1: activations / outputs move as ONE 5-d box per tile whose traversal order is
                                // (8-channel group, 64-pixel block, channel, pixel): the TMA unit touches 8 channel
@@ -201,9 +198,8 @@ pw_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
                         (it / kchunks) * p.Mpad + mb * 128);
       }
       int s = 0, ph = 0;
-      for (int tl = 0;; ++tl) {
-        const int t = ((tl / p.tgroup) * gridDim.x + blockIdx.x) * p.tgroup + tl % p.tgroup;
-        if ((tl / p.tgroup) * gridDim.x * p.tgroup >= p.num_tiles) break;
+      for (int tl = 0; tl * (int)gridDim.x < p.num_tiles; ++tl) {   // the consumers' tile order
+        const int t = tl * gridDim.x + blockIdx.x;
         if (t >= p.num_tiles) continue;
         const int mg = t % p.num_mg;
         const int tt = t / p.num_mg;
@@ -250,9 +246,10 @@ pw_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
     float acc[MB][BN / 2];
     if (p.wres) mbar_wait(wfull, 0);
     int s = 0, ph = 0, ob = 0;
-    for (int tl = 0;; ++tl) {
-      const int t = ((tl / p.tgroup) * gridDim.x + blockIdx.x) * p.tgroup + tl % p.tgroup;
-      if ((tl / p.tgroup) * gridDim.x * p.tgroup >= p.num_tiles) break;
+    // tiles blockIdx.x + k gridDim.x, counted in rounds: the loop `t += gridDim.x` costs pw_gemm_kernel<2> a register
+    // spill in the epilogue
+    for (int tl = 0; tl * (int)gridDim.x < p.num_tiles; ++tl) {
+      const int t = tl * gridDim.x + blockIdx.x;
       if (t >= p.num_tiles) continue;
       const int mg = t % p.num_mg;
       const int tt = t / p.num_mg;
@@ -339,24 +336,6 @@ pw_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
 }
 
 inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
-// tuning knob: positive integer from the environment, else `dflt`
-// Every knob is read from the environment ONCE per process (getenv on the launch path showed up in the
-// N=8 step, which is CPU-bound): a small table keyed by the name's address (names are string literals).
-struct EnvKnob { const char* name; const char* val; };
-EnvKnob g_env_tab[32];
-int g_env_n = 0;
-inline const char* env_get(const char* name) {
-  for (int i = 0; i < g_env_n; ++i)
-    if (g_env_tab[i].name == name) return g_env_tab[i].val;
-  const char* v = getenv(name);
-  if (g_env_n < 32) { g_env_tab[g_env_n].name = name; g_env_tab[g_env_n].val = v; ++g_env_n; }
-  return v;
-}
-inline int env_int(const char* name, int dflt) {
-  const char* e = env_get(name);
-  const int v = e ? atoi(e) : 0;
-  return v > 0 ? v : dflt;
-}
 inline int sm_count() {
   static int sms = 0;
   if (!sms) {
@@ -378,7 +357,6 @@ int launch_pw(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& t
   const int wres_bytes = p.taps * kchunks * MB * A_BLK_BYTES;
   const int sms = sm_count();
   const int grid = p.num_tiles < sms ? p.num_tiles : sms;
-  if (p.num_tiles < 16 * sms) p.tgroup = 1;   // small problems: keep every SM busy
   // stationary weights: only with one group of output channels (every CTA then needs the same filter rows)
   p.wres = (wres_bytes <= 128 * 1024 && p.num_mg == 1) ? 1 : 0;
   const int stage_bytes = (p.wres ? 0 : MB * A_BLK_BYTES) + (BN / 64) * B_BLK_BYTES;
@@ -457,7 +435,7 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
   const int nt = (c.px && taps == 1) ? px_tile_channels(c.M) : 0;
   const bool px = nt && (long long)c.N * ((P + BN - 1) / BN) >= 2ll * sm_count();
   const int Mpad = round_up(c.M, px ? nt : 128), Cpad = round_up(c.Cin, BK);
-  const bool v2 = taps > 1 && !env_get("SPC_TAP_V1") && tap_v2_supported(c.M, c.Cin, c.R, c.S, c.H, c.W, c.N, cs);
+  const bool v2 = taps > 1 && tap_v2_supported(c.M, c.Cin, c.R, c.S, c.H, c.W, c.N, cs);
   const bool copies = (c.S > 1 || cs > 1) && taps > 1 && !v2;   // column-shifted (and subsampled) copies of the input
   const uintptr_t ws0 = reinterpret_cast<uintptr_t>(ws);
   const uintptr_t wp_addr = (ws0 + 1023) & ~(uintptr_t)1023;
@@ -487,12 +465,10 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
     xsrc = reinterpret_cast<const __nv_bfloat16*>(xs);
   }
   CUtensorMap tw, tx, tx4, ty;
-  // 5-d boxes (see PwParams::x5) for the layers whose channel planes span several 2 MB pages (from 4 MB planes).
-  // SPC_PW_BOX5 = 0..3 overrides (bit 0: activations, bit 1: outputs).
-  const char* box5_env = env_get("SPC_PW_BOX5");
-  const int box5 = box5_env ? atoi(box5_env) : ((size_t)P * 2 >= ((size_t)4 << 20) ? 3 : 0);
-  const int x5 = (taps == 1 && cs == 1 && (box5 & 1) && P % 64 == 0 && c.Cin % 8 == 0) ? 1 : 0;
-  const int y5 = (taps == 1 && (box5 & 2) && P % 64 == 0 && c.M % 8 == 0) ? 1 : 0;
+  // 5-d boxes (see PwParams::x5) for the layers whose channel planes span several 2 MB pages (from 4 MB planes)
+  const bool box5 = (size_t)P * 2 >= ((size_t)4 << 20);
+  const int x5 = (taps == 1 && cs == 1 && box5 && P % 64 == 0 && c.Cin % 8 == 0) ? 1 : 0;
+  const int y5 = (taps == 1 && box5 && P % 64 == 0 && c.M % 8 == 0) ? 1 : 0;
   {
     const uint64_t dims[2] = {(uint64_t)Cpad, (uint64_t)taps * Mpad};
     const uint64_t strides[2] = {0, (uint64_t)Cpad * 2};
@@ -529,11 +505,6 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
   p.taps = taps; p.S = c.S; p.ph = c.ph; p.pw = c.pw; p.W = Wo; p.Mpad = Mpad;
   p.shiftN = copies ? c.N : 0;
   p.rowmul = cs;
-  {
-    const char* e = env_get("SPC_TILE_GROUP");
-    p.tgroup = e ? atoi(e) : 1;
-    if (p.tgroup < 1) p.tgroup = 1;
-  }
   // groups of at most two 128-row blocks of output channels: a consumer thread holds 64 fp32 accumulators per block
   const int MBtot = Mpad / 128;
   const int mb = MBtot >= 2 ? 2 : 1;
@@ -582,8 +553,6 @@ struct WgParams {
   int rowmul;       // input row = rowmul * output row + tap row offset
   int mrows;        // dY rows per 128-row block (<= 128): K split EVENLY over its blocks, so every item streams the
                     // same number of valid rows and the CTAs that share an x chunk stay in lock-step (L2 hits)
-  int split_major;  // 1: concurrently running CTAs cover all (m-group, channel-block, pass) groups of the SAME
-                    //    pixel range, so the dY / x chunks every group re-reads come from L2, not HBM
   int pb;           // 64-pixel blocks per stage (1, or 2 = "wide" stages for 1x1 layers with multi-page channel planes)
   int dy5, x5;      // wide stages: operand moves as one 5-d box [8-ch group][px block][8 ch][128 B] (see PwParams::x5)
 };
@@ -612,10 +581,11 @@ pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_consta
   const int num_items = ngroups * p.splits;
   const int per_split = (p.chunks_total + p.splits - 1) / p.splits;
 
-  // item -> (split, tap pass, channel block, m group)
+  // item -> (split, tap pass, channel block, m group), split-major: concurrently running CTAs cover all (m group,
+  // channel block, pass) groups of the SAME pixel range, so the dY / x chunks every group re-reads come from L2, not HBM
 #define WG_DECODE(it)                                                        \
-  const int sp = p.split_major ? (it) / ngroups : (it) % p.splits;           \
-  const int g_ = p.split_major ? (it) % ngroups : (it) / p.splits;           \
+  const int sp = (it) / ngroups;                                             \
+  const int g_ = (it) % ngroups;                                             \
   const int pass = g_ % p.passes;                                            \
   const int nb = (g_ / p.passes) % p.n_blocks;                               \
   const int mgp = g_ / (p.passes * p.n_blocks);                              \
@@ -768,7 +738,6 @@ int launch_wg(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMap& 
   const int stage_bytes = p.pb * (p.MG * A_BLK_BYTES + TG * b_slot);
   p.stages = (SMEM_LIMIT - SMEM_AUX) / stage_bytes;
   if (p.stages > 6) p.stages = 6;
-  p.stages = min(p.stages, env_int("SPC_WG_STAGES", p.stages));
   SPC_REQUIRE(p.stages >= 2, "wgmma wgrad: smem budget");
   const int sms = sm_count();
   const int groups = p.mgroups * p.n_blocks * p.passes;
@@ -794,11 +763,7 @@ int launch_wg(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMap& 
       if (t < best * 0.98) { best = t; splits = s; }
     }
   }
-  splits = env_int("SPC_WG_SPLITS", splits);
-  if (splits > p.chunks_total / 8) splits = p.chunks_total / 8;
-  if (splits < 1) splits = 1;
   p.splits = splits;
-  p.split_major = env_get("SPC_WG_GROUP_MAJOR") ? 0 : 1;            // A/B knob: previous item order
   const int smem = p.stages * stage_bytes + SMEM_AUX;
   auto kern = pw_wgrad_kernel<NBLK, NA>;
   static bool attr_set = false;
@@ -847,31 +812,24 @@ int run_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, int K,
     p.nblk = w <= 16 ? 16 : (w <= 32 ? 32 : (w <= 64 ? 64 : 128));
   }
   int MBtot = (K + 127) / 128;
-  p.mrows = env_get("SPC_WG_ROWS128") ? 128 : round_up((K + MBtot - 1) / MBtot, 8);   // e.g. K = 416 -> 4 blocks of 104
+  p.mrows = round_up((K + MBtot - 1) / MBtot, 8);   // e.g. K = 416 -> 4 blocks of 104
   MBtot = (K + p.mrows - 1) / p.mrows;
   int MG = p.taps > 1 ? 1 : WG_ACC / p.nblk;
   if (MG > MBtot) MG = MBtot;
-  MG = min(MG, env_int("SPC_WG_MG", MG));
   MG = MG >= 4 ? 4 : (MG >= 2 ? 2 : 1);
   p.chunks_per_image = (P + 63) / 64;
   p.chunks_total = p.chunks_per_image * N;
   p.pb = 1;
   // wide stages (two 64-pixel blocks per operand row and stage, 5-d boxes): for 1x1 layers whose channel planes span
-  // several 2 MB pages, same reason as PwParams::x5.  SPC_WG_WIDE=0/1 overrides, SPC_WG_BOX5 (bit 0 dy, bit 1 x).
-  {
-    const char* we = env_get("SPC_WG_WIDE");
-    const bool wide = p.taps == 1 && P % 128 == 0 && (we ? atoi(we) != 0 : (size_t)P * 2 >= ((size_t)2 << 20));
-    if (wide) {
-      const int b_slot = (p.nblk * 128 + 1023) & ~1023;
-      while (MG > 1 && 2 * 2 * (MG * A_BLK_BYTES + b_slot) > SMEM_LIMIT - SMEM_AUX) MG >>= 1;
-      p.pb = 2;
-      p.chunks_per_image = P / 128;
-      p.chunks_total = p.chunks_per_image * N;
-      const char* be = env_get("SPC_WG_BOX5");
-      const int b5 = be ? atoi(be) : 3;
-      p.dy5 = ((b5 & 1) && K % 8 == 0 && p.mrows % 8 == 0) ? 1 : 0;
-      p.x5 = ((b5 & 2) && C % 8 == 0) ? 1 : 0;
-    }
+  // several 2 MB pages, same reason as PwParams::x5
+  if (p.taps == 1 && P % 128 == 0 && (size_t)P * 2 >= ((size_t)2 << 20)) {
+    const int b_slot = (p.nblk * 128 + 1023) & ~1023;
+    while (MG > 1 && 2 * 2 * (MG * A_BLK_BYTES + b_slot) > SMEM_LIMIT - SMEM_AUX) MG >>= 1;
+    p.pb = 2;
+    p.chunks_per_image = P / 128;
+    p.chunks_total = p.chunks_per_image * N;
+    p.dy5 = K % 8 == 0 ? 1 : 0;   // mrows is a multiple of 8
+    p.x5 = C % 8 == 0 ? 1 : 0;
   }
   p.MG = MG;
   p.mgroups = (MBtot + MG - 1) / MG;
@@ -1187,10 +1145,9 @@ size_t tc_workspace_bytes(const spc_conv_desc* d, int op) {
     b += align1k(2ull * d->N * d->K * Ho * Wo * 2) + align1k(4ull * d->N * d->C * Ho * Wo * 2) + 4096;
     return b;
   }
-  if (op != 2 && !env_get("SPC_TAP_V1") &&
-      tap_v2_supported(op == 1 ? d->C : d->K, op == 1 ? d->K : d->C, d->R, d->S, d->H, d->W, d->N, cs))
+  if (op != 2 && tap_v2_supported(op == 1 ? d->C : d->K, op == 1 ? d->K : d->C, d->R, d->S, d->H, d->W, d->N, cs))
     return b;               // conv_tap.cu forms the horizontal taps in shared memory: no copies
-  if (op == 2 && !env_get("SPC_TAP_V1") && wgrad_tap_supported(d->K, d->C, d->R, d->S, d->H, d->W, cs))
+  if (op == 2 && wgrad_tap_supported(d->K, d->C, d->R, d->S, d->H, d->W, cs))
     return b;               // wgrad_tap.cu likewise
   if (d->S > 1 || cs > 1)   // S column-shifted (stride 2: also subsampled) copies of the conv input
     b += align1k((size_t)d->S * d->N * (op == 1 ? d->K : d->C) * d->H * Wo * 2) + 2048;
@@ -1278,15 +1235,14 @@ int tc_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* d
                 d->H * d->W, ws, ws_bytes, st);
 }
 
-int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, int accumulate, void* ws,
-                  size_t ws_bytes, cudaStream_t st) {
-  // the kernel accumulates with atomics; api.cu has already zeroed dw when !accumulate
-  (void)accumulate;
+int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void* ws, size_t ws_bytes,
+                  cudaStream_t st) {
+  // the kernels accumulate into dw with atomics; api.cu has zeroed it unless the caller accumulates
   const __nv_bfloat16* xb = reinterpret_cast<const __nv_bfloat16*>(x);
   const __nv_bfloat16* dyb = reinterpret_cast<const __nv_bfloat16*>(dy);
   if (d->R * d->S > 1) {
     const int cs = d->stride_h;
-    if (!env_get("SPC_TAP_V1") && wgrad_tap_supported(d->K, d->C, d->R, d->S, d->H, d->W, cs))
+    if (wgrad_tap_supported(d->K, d->C, d->R, d->S, d->H, d->W, cs))
       return run_wgrad_tap(xb, dyb, dw, d->K, d->C, d->N, d->H, d->W, d->R, d->S, st);
     const bool copies = d->S > 1 || cs > 1;
     if (copies) {
@@ -1332,6 +1288,3 @@ int make_tmap_ex(CUtensorMap* m, const void* base, int rank, const uint64_t* dim
 int tc_sm_count() { return sm_count(); }
 
 }  // namespace spc
-
-// tuning probes change SPC_* knobs inside one process: forget the cached values
-extern "C" void spc_reload_env(void) { spc::g_env_n = 0; }

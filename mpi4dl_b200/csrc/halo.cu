@@ -96,46 +96,21 @@ __global__ void halo_crop_kernel(const T* __restrict__ dy, T* __restrict__ dx, i
   }
 }
 
-__global__ void mailbox_signal_kernel(uint32_t* flag, uint32_t seq) {
-  __threadfence_system();
-  asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(flag), "r"(seq) : "memory");
-}
-
-__global__ void mailbox_wait_kernel(const uint32_t* flag, uint32_t seq, unsigned long long timeout_ns) {
-  uint32_t v;
-  unsigned long long t0;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-  do {
-    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
-    if ((int32_t)(v - seq) >= 0) break;
-    __nanosleep(64);
-    if (timeout_ns) {
-      unsigned long long t;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      if (t - t0 > timeout_ns) {
-        printf("libspconv: mailbox wait timed out (have %u, want %u) -- trapping\n", v, seq);
-        __trap();
-      }
-    }
-  } while (true);
-}
-
 // ---- fused protocol kernels -----------------------------------------------------------------
 // post:    wait until every neighbour has drained the slot we are about to overwrite (ack flags,
 //          local memory) -> pack all strips straight into the neighbours' slots (peer stores) ->
 //          the LAST block publishes the sequence number on the neighbours' arrival flags.
 // collect: wait for the neighbours' arrival flags -> copy the received strips out of the mailbox
 //          into private buffers (they are needed again by wgrad) -> the last block acks.
+// Graph-capturable: no host-side state in the launch arguments.  The sequence number of the exchange is *seq_word + 1;
+// its parity selects the half of the double-buffered slot (payload pointers advance by par_bytes) and the flag bank
+// (flag pointers advance by 9 words).  wait_lag: 0 = wait for the current sequence (arrivals), 2 = wait for
+// sequence-2 (acks of the slot half about to be overwritten).
 struct FlagSet {
-  uint32_t* wait[9];     // flags to wait on (>= wait_seq), NULL = skip
-  uint32_t* signal[9];   // flags to publish `seq` on when the whole grid is done, NULL = skip
-  uint32_t wait_seq, seq;
+  uint32_t* wait[9];     // flags to wait on (>= sequence - wait_lag), NULL = skip
+  uint32_t* signal[9];   // flags to publish the sequence number on when the whole grid is done, NULL = skip
   unsigned int* counter; // grid completion counter (device memory, self-resetting)
-  // "auto" mode (graph-capturable: no host-side state in the launch arguments): the sequence number of the
-  // exchange is *seq_word + 1; its parity selects the half of the double-buffered slot (payload pointers
-  // advance by par_bytes) and the flag bank (flag pointers advance by 9 words).  wait_lag: 0 = wait for the
-  // current sequence (arrivals), 2 = wait for sequence-2 (acks of the slot half about to be overwritten).
-  uint32_t* seq_word;    // NULL = immediate mode (wait_seq / seq above)
+  uint32_t* seq_word;
   int advance_seq;       // the last block stores the new sequence number (collect = end of the exchange)
   int wait_lag;
   long long par_bytes;
@@ -150,13 +125,9 @@ __device__ __forceinline__ unsigned long long global_ns() {
 
 // returns the sequence number of this exchange; threads 0..8 wait for their direction's flag
 __device__ __forceinline__ uint32_t wait_flags(const FlagSet& f) {
-  uint32_t seq = f.seq, wseq = f.wait_seq;
-  int par = 0;
-  if (f.seq_word) {
-    seq = *reinterpret_cast<const volatile uint32_t*>(f.seq_word) + 1u;
-    par = (int)(seq & 1u);
-    wseq = f.wait_lag ? (seq > (uint32_t)f.wait_lag ? seq - (uint32_t)f.wait_lag : 0u) : seq;
-  }
+  const uint32_t seq = *reinterpret_cast<const volatile uint32_t*>(f.seq_word) + 1u;
+  const int par = (int)(seq & 1u);
+  const uint32_t wseq = f.wait_lag ? (seq > (uint32_t)f.wait_lag ? seq - (uint32_t)f.wait_lag : 0u) : seq;
   if (threadIdx.x < 9) {
     const uint32_t* w = f.wait[threadIdx.x];
     if (w != nullptr && wseq != 0u) {
@@ -187,12 +158,12 @@ __device__ __forceinline__ void signal_when_grid_done(const FlagSet& f, uint32_t
     const unsigned int done = atomicAdd(f.counter, 1u);
     if (done == gridDim.x - 1) {   // every block has fenced its stores
       __threadfence_system();
-      const int par = f.seq_word ? (int)(seq & 1u) : 0;
+      const int par = (int)(seq & 1u);
       for (int i = 0; i < 9; ++i)
         if (f.signal[i])
           asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(f.signal[i] + par * 9), "r"(seq) : "memory");
       *f.counter = 0u;
-      if (f.seq_word && f.advance_seq) *reinterpret_cast<volatile uint32_t*>(f.seq_word) = seq;
+      if (f.advance_seq) *reinterpret_cast<volatile uint32_t*>(f.seq_word) = seq;
     }
   }
 }
@@ -200,7 +171,7 @@ __device__ __forceinline__ void signal_when_grid_done(const FlagSet& f, uint32_t
 template <typename T>
 __global__ void halo_post_kernel(const PackParams p, const FlagSet f) {
   const uint32_t seq = wait_flags(f);
-  const long long pofs = f.seq_word ? (long long)(seq & 1u) * f.par_bytes : 0;   // slot half of this sequence number
+  const long long pofs = (long long)(seq & 1u) * f.par_bytes;   // slot half of this sequence number
   const long long total = p.off[9];
   const T* x = reinterpret_cast<const T*>(p.x);
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -232,7 +203,7 @@ struct CollectParams {
 // caller-given (fp32) strip buffers src[d] copied into the neighbours' slots dst[d], instead of a pack of the tile.
 __global__ void halo_post_strips_kernel(const CollectParams p, const FlagSet f) {
   const uint32_t seq = wait_flags(f);
-  const long long pofs = f.seq_word ? (long long)(seq & 1u) * f.par_bytes : 0;
+  const long long pofs = (long long)(seq & 1u) * f.par_bytes;
   const long long total = p.off[9] / 4;   // 4-byte units
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
@@ -248,7 +219,7 @@ __global__ void halo_post_strips_kernel(const CollectParams p, const FlagSet f) 
 
 __global__ void halo_collect_kernel(const CollectParams p, const FlagSet f) {
   const uint32_t seq = wait_flags(f);
-  const long long pofs = f.seq_word ? (long long)(seq & 1u) * f.par_bytes : 0;
+  const long long pofs = (long long)(seq & 1u) * f.par_bytes;
   const long long total = p.off[9] / 2;   // 2-byte units (strips of bf16 columns may be 2-byte sized)
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
@@ -439,7 +410,10 @@ int spc_halo_crop(int N, int C, int H, int W, int halo_h, int halo_w, int dtype,
   return SPC_OK;
 }
 
-static uint32_t* mb_flag(spc_mailbox* mb, int idx);
+// flag word idx of a mailbox: the flags follow the data area
+static uint32_t* mb_flag(spc_mailbox* mb, int idx) {
+  return reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(mb->base) + mb->bytes) + idx;
+}
 
 // spin bound of the flag waits: SPCONV_SPIN_TIMEOUT_S seconds (default 120; 0 = spin forever)
 static unsigned long long spin_timeout_ns() {
@@ -452,37 +426,34 @@ static unsigned long long spin_timeout_ns() {
   return (unsigned long long)v;
 }
 
-// shared by the immediate and the auto-sequence entry points.  seq_idx < 0: immediate mode.
-static int halo_post_impl(int N, int C, int H, int W, int halo_h, int halo_w, int dtype, const void* x,
-                          void* const send[9], size_t slot_bytes, spc_mailbox* self, spc_mailbox* const peers[9],
-                          const int ack_idx[9], uint32_t ack_seq, const int arrival_idx[9], uint32_t seq, int seq_idx,
-                          int counter_idx, void* stream) {
-  SPC_REQUIRE(x && send && self && peers && ack_idx && arrival_idx, "halo_post: null pointer");
+int spc_halo_post_auto(int N, int C, int H, int W, int halo_h, int halo_w, int dtype, const void* x,
+                       void* const send0[9], size_t slot_bytes, spc_mailbox* self, spc_mailbox* const peers[9],
+                       const int ack_idx0[9], const int arrival_idx0[9], int seq_idx, int counter_idx, void* stream) {
+  SPC_REQUIRE(self && seq_idx >= 0 && seq_idx < self->nflags && counter_idx >= 0 && counter_idx < self->nflags,
+              "halo_post_auto: bad sequence / counter flag index");
+  SPC_REQUIRE(x && send0 && peers && ack_idx0 && arrival_idx0, "halo_post: null pointer");
   spc::PackParams p{};
   p.x = x; p.N = N; p.C = C; p.H = H; p.W = W; p.hh = halo_h; p.hw = halo_w;
   spc::FlagSet f{};
-  const bool autoseq = seq_idx >= 0;
   long long off = 0;
   for (int d = 0; d < 9; ++d) {
     p.off[d] = off;
-    p.send[d] = (d == 4) ? nullptr : send[d];
+    p.send[d] = (d == 4) ? nullptr : send0[d];
     if (p.send[d]) {
       SPC_REQUIRE(peers[d] != nullptr, "halo_post: no peer mailbox for direction %d", d);
       const long long sh = (d / 3 == 1) ? H : halo_h, sw = (d % 3 == 1) ? W : halo_w;
       off += (long long)N * C * sh * sw;
-      f.wait[d] = (autoseq || ack_seq) ? mb_flag(self, ack_idx[d]) : nullptr;
-      f.signal[d] = mb_flag(peers[d], arrival_idx[d]);
+      f.wait[d] = mb_flag(self, ack_idx0[d]);
+      f.signal[d] = mb_flag(peers[d], arrival_idx0[d]);
     }
   }
   p.off[9] = off;
   if (off == 0) return SPC_OK;
-  f.wait_seq = ack_seq; f.seq = seq;
-  f.seq_word = autoseq ? mb_flag(self, seq_idx) : nullptr;
+  f.seq_word = mb_flag(self, seq_idx);
   f.advance_seq = 0; f.wait_lag = 2; f.par_bytes = (long long)slot_bytes;
   f.timeout_ns = spin_timeout_ns();
-  // per-slot completion counter (two streams may run exchanges of different layers concurrently);
-  // counter_idx < 0: the mailbox-wide spare word
-  f.counter = reinterpret_cast<unsigned int*>(mb_flag(self, counter_idx >= 0 ? counter_idx : self->nflags));
+  // per-slot completion counter (two streams may run exchanges of different layers concurrently)
+  f.counter = reinterpret_cast<unsigned int*>(mb_flag(self, counter_idx));
   const int grid = spc::grid_for(off) > 64 ? 64 : spc::grid_for(off);
   if (dtype == SPC_BF16) spc::halo_post_kernel<__nv_bfloat16><<<grid, 256, 0, (cudaStream_t)stream>>>(p, f);
   else spc::halo_post_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(p, f);
@@ -491,67 +462,37 @@ static int halo_post_impl(int N, int C, int H, int W, int halo_h, int halo_w, in
   return SPC_OK;
 }
 
-static int halo_collect_impl(void* const dst[9], const void* const src[9], const size_t bytes[9], size_t slot_bytes,
-                             spc_mailbox* self, spc_mailbox* const peers[9], const int arrival_idx[9], uint32_t seq,
-                             const int ack_idx[9], int seq_idx, int counter_idx, void* stream) {
-  SPC_REQUIRE(dst && src && bytes && self && peers, "halo_collect: null pointer");
+int spc_halo_collect_auto(void* const dst[9], const void* const src0[9], const size_t bytes[9], size_t slot_bytes,
+                          spc_mailbox* self, spc_mailbox* const peers[9], const int arrival_idx0[9],
+                          const int ack_idx0[9], int seq_idx, int counter_idx, void* stream) {
+  SPC_REQUIRE(self && seq_idx >= 0 && seq_idx < self->nflags && counter_idx >= 0 && counter_idx < self->nflags,
+              "halo_collect_auto: bad sequence / counter flag index");
+  SPC_REQUIRE(dst && src0 && bytes && peers, "halo_collect: null pointer");
   spc::CollectParams p{};
   spc::FlagSet f{};
   long long off = 0;
   for (int d = 0; d < 9; ++d) {
     p.off[d] = off;
     if (d != 4 && dst[d] && bytes[d]) {
-      SPC_REQUIRE(peers[d] != nullptr && src[d] != nullptr, "halo_collect: missing source for direction %d", d);
+      SPC_REQUIRE(peers[d] != nullptr && src0[d] != nullptr, "halo_collect: missing source for direction %d", d);
       p.dst[d] = reinterpret_cast<uint8_t*>(dst[d]);
-      p.src[d] = reinterpret_cast<const uint8_t*>(src[d]);
+      p.src[d] = reinterpret_cast<const uint8_t*>(src0[d]);
       off += (long long)bytes[d];
-      f.wait[d] = mb_flag(self, arrival_idx[d]);
-      f.signal[d] = mb_flag(peers[d], ack_idx[d]);
+      f.wait[d] = mb_flag(self, arrival_idx0[d]);
+      f.signal[d] = mb_flag(peers[d], ack_idx0[d]);
     }
   }
   p.off[9] = off;
   if (off == 0) return SPC_OK;
-  f.wait_seq = seq; f.seq = seq;
-  f.seq_word = seq_idx >= 0 ? mb_flag(self, seq_idx) : nullptr;
+  f.seq_word = mb_flag(self, seq_idx);
   f.advance_seq = 1; f.wait_lag = 0; f.par_bytes = (long long)slot_bytes;
   f.timeout_ns = spin_timeout_ns();
-  f.counter = reinterpret_cast<unsigned int*>(mb_flag(self, counter_idx >= 0 ? counter_idx : self->nflags + 1));
+  f.counter = reinterpret_cast<unsigned int*>(mb_flag(self, counter_idx));
   const int grid = spc::grid_for((size_t)off / 2) > 64 ? 64 : spc::grid_for((size_t)off / 2);
   spc::halo_collect_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p, f);
   spc::count_launch();
   SPC_CHECK_CUDA(cudaGetLastError());
   return SPC_OK;
-}
-
-int spc_halo_post(int N, int C, int H, int W, int halo_h, int halo_w, int dtype, const void* x, void* const send[9],
-                  spc_mailbox* self, spc_mailbox* const peers[9], const int ack_idx[9], uint32_t ack_seq,
-                  const int arrival_idx[9], uint32_t seq, void* stream) {
-  return halo_post_impl(N, C, H, W, halo_h, halo_w, dtype, x, send, 0, self, peers, ack_idx, ack_seq, arrival_idx, seq, -1,
-                        -1, stream);
-}
-
-int spc_halo_collect(void* const dst[9], const void* const src[9], const size_t bytes[9], spc_mailbox* self,
-                     spc_mailbox* const peers[9], const int arrival_idx[9], uint32_t seq, const int ack_idx[9],
-                     void* stream) {
-  return halo_collect_impl(dst, src, bytes, 0, self, peers, arrival_idx, seq, ack_idx, -1, -1, stream);
-}
-
-int spc_halo_post_auto(int N, int C, int H, int W, int halo_h, int halo_w, int dtype, const void* x,
-                       void* const send0[9], size_t slot_bytes, spc_mailbox* self, spc_mailbox* const peers[9],
-                       const int ack_idx0[9], const int arrival_idx0[9], int seq_idx, int counter_idx, void* stream) {
-  SPC_REQUIRE(self && seq_idx >= 0 && seq_idx < self->nflags && counter_idx >= 0 && counter_idx < self->nflags,
-              "halo_post_auto: bad sequence / counter flag index");
-  return halo_post_impl(N, C, H, W, halo_h, halo_w, dtype, x, send0, slot_bytes, self, peers, ack_idx0, 0, arrival_idx0, 0,
-                        seq_idx, counter_idx, stream);
-}
-
-int spc_halo_collect_auto(void* const dst[9], const void* const src0[9], const size_t bytes[9], size_t slot_bytes,
-                          spc_mailbox* self, spc_mailbox* const peers[9], const int arrival_idx0[9],
-                          const int ack_idx0[9], int seq_idx, int counter_idx, void* stream) {
-  SPC_REQUIRE(self && seq_idx >= 0 && seq_idx < self->nflags && counter_idx >= 0 && counter_idx < self->nflags,
-              "halo_collect_auto: bad sequence / counter flag index");
-  return halo_collect_impl(dst, src0, bytes, slot_bytes, self, peers, arrival_idx0, 0, ack_idx0, seq_idx, counter_idx,
-                           stream);
 }
 
 int spc_halo_post_strips_auto(const void* const src[9], const size_t bytes[9], void* const send0[9], size_t slot_bytes,
@@ -595,7 +536,7 @@ int spc_mailbox_create(spc_mailbox** out, size_t bytes, int nflags) {
   SPC_REQUIRE(out && nflags >= 0, "mailbox_create: bad arguments");
   spc_mailbox* mb = new spc_mailbox();
   mb->bytes = mb_round(bytes); mb->nflags = nflags; mb->owner = 1; mb->base = nullptr;
-  const size_t total = mb->bytes + mb_round(sizeof(uint32_t) * (size_t)nflags) + 256;
+  const size_t total = mb->bytes + mb_round(sizeof(uint32_t) * (size_t)nflags);
   cudaError_t e = cudaMalloc(&mb->base, total);  // plain cudaMalloc: IPC-exportable
   if (e != cudaSuccess) {
     spc::set_error("mailbox_create: cudaMalloc(%zu) failed: %s", total, cudaGetErrorString(e));
@@ -634,26 +575,6 @@ int spc_mailbox_open(spc_mailbox** out, const unsigned char handle[SPC_IPC_HANDL
   spc_mailbox* mb = new spc_mailbox();
   mb->base = p; mb->bytes = mb_round(bytes); mb->nflags = nflags; mb->owner = 0;
   *out = mb;
-  return SPC_OK;
-}
-
-static uint32_t* mb_flag(spc_mailbox* mb, int idx) {   // idx may be nflags / nflags+1: two spare counter words
-  return reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(mb->base) + mb->bytes) + idx;
-}
-
-int spc_mailbox_signal(spc_mailbox* peer_mb, int idx, uint32_t seq, void* stream) {
-  SPC_REQUIRE(peer_mb && idx >= 0 && idx < peer_mb->nflags, "mailbox_signal: bad flag index %d", idx);
-  spc::mailbox_signal_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(mb_flag(peer_mb, idx), seq);
-  spc::count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  return SPC_OK;
-}
-
-int spc_mailbox_wait(spc_mailbox* mb, int idx, uint32_t seq, void* stream) {
-  SPC_REQUIRE(mb && idx >= 0 && idx < mb->nflags, "mailbox_wait: bad flag index %d", idx);
-  spc::mailbox_wait_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(mb_flag(mb, idx), seq, spin_timeout_ns());
-  spc::count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
   return SPC_OK;
 }
 

@@ -1,8 +1,12 @@
-"""CPU-only: libspconv.so loads and exports every symbol include/spconv.h declares; argument
+"""CPU-only: libspconv.so loads and exports exactly the spc_* symbols include/spconv.h declares; argument
 validation works without a GPU (no compute calls here)."""
 import ctypes as C
 import os
 import re
+import shutil
+import subprocess
+
+import pytest
 
 from mpi4dl_b200 import _lib
 
@@ -26,10 +30,21 @@ def test_library_exports_every_declared_symbol():
     assert bound == set(names)
 
 
-def test_version_101_and_structs():
-    """SPC_VERSION 101: spc_bn_stats returns mean and variance and, with spc_bn_bwd_reduce, takes a workspace"""
+def test_library_exports_only_declared_symbols():
+    """an entry point removed from spconv.h does not stay behind as an undeclared export"""
+    if shutil.which("nm") is None:
+        pytest.skip("nm (binutils) is not installed")
+    out = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
+    exported = {ln.split()[-1] for ln in out.splitlines() if ln.split() and ln.split()[-1].startswith("spc_")}
+    assert exported == set(_declared()), "exported but not declared: %s; declared but not exported: %s" % (
+        sorted(exported - set(_declared())), sorted(set(_declared()) - exported))
+
+
+def test_version_102_and_structs():
+    """SPC_VERSION 102: the immediate-mode halo protocol (spc_halo_post / spc_halo_collect, spc_mailbox_signal /
+    spc_mailbox_wait) and spc_reload_env are gone"""
     L = _lib.lib()
-    assert L.spc_version() == 101
+    assert L.spc_version() == 102
     assert C.sizeof(_lib.ConvDesc) == 13 * 4
     assert C.sizeof(_lib.PoolDesc) == 9 * 4
     assert C.sizeof(_lib.Halo) == 9 * C.sizeof(C.c_void_p)

@@ -63,6 +63,8 @@ CASES = [
     Case(13, 29, 7, 1, 1, 2, 9, 64, True,
          K("conv_tap_kernel<2, 1, 1>", "conv_tap_kernel<2, 1, 2>", "pw_wgrad_kernel<16, 8>", "repack_weights_kernel"),
          "odd H (last 2-row tile half outside); resident weights; wgrad 7 taps on 8 accumulators (one spare)"),
+    Case(136, 136, 3, 1, 1, 1, 4, 64, False, K("pw_gemm_kernel<2>", "pw_wgrad_kernel<128, 2>"),
+         "M = 136 > 128 both ways: fprop and dgrad on pw_gemm_kernel in tap mode (row-shifted boxes, no copies)"),
     Case(45, 61, 5, 1, 1, 2, 12, 128, False,
          K("conv_tap_kernel<2, 1, 3>", "conv_tap_kernel<2, 1, 4>", "pw_wgrad_kernel<64, 4>"),
          "wgrad TG=4: passes of 4 + 1 taps (3 spare)"),
@@ -94,6 +96,9 @@ CASES = [
          K("shift_copies_vec_kernel<3, 1>", "pw_gemm_kernel<2>", "conv_tap_kernel<2, 3, 4>", "pw_wgrad_kernel<16, 16>"),
          "M = 200 > 128: fprop on shifted copies; dgrad 4 k-chunks, the last 8 of 64 channels; "
          "wgrad K > 128: copies + NA=16 with 9 taps (7 spare)"),
+    Case(136, 136, 3, 3, 1, 1, 4, 64, False,
+         K("shift_copies_vec_kernel<3, 1>", "pw_gemm_kernel<2>", "pw_wgrad_kernel<128, 2>"),
+         "136 channels both ways: every op on shifted copies; wgrad passes of 2 taps (last 1)"),
     # ---- S = 5
     Case(29, 13, 5, 5, 1, 2, 7, 64, True,
          K("conv_tap_kernel<2, 5, 2>", "conv_tap_kernel<2, 5, 1>", "wgrad_tap_kernel<5, 16>"),
@@ -116,6 +121,9 @@ CASES = [
            "pw_wgrad_kernel<32, 8>"),
          "fprop streamed weights with group=1; 5x5 at QC=32 has no wgrad_tap plan: copies + 25 taps in passes of 8 "
          "(last 1)"),
+    Case(136, 136, 1, 5, 1, 1, 3, 64, False,
+         K("shift_copies_vec_kernel<5, 2>", "pw_gemm_kernel<2>", "pw_wgrad_kernel<128, 2>"),
+         "136 channels both ways: every op on shifted copies"),
     # ---- S = 7
     Case(29, 13, 3, 7, 1, 2, 7, 64, False,
          K("conv_tap_kernel<2, 7, 2>", "conv_tap_kernel<2, 7, 1>", "wgrad_tap_kernel<7, 16>"),
@@ -135,6 +143,9 @@ CASES = [
     Case(128, 128, 3, 7, 1, 1, 5, 64, False,
          K("conv_tap_kernel<2, 7, 4>", "shift_copies_vec_kernel<7, 3>", "pw_wgrad_kernel<128, 2>"),
          "21 taps x 2 k-chunks: streamed weights; no wgrad_tap plan: copies + passes of 2 taps (last 1)"),
+    Case(136, 136, 1, 7, 1, 1, 3, 64, False,
+         K("shift_copies_vec_kernel<7, 3>", "pw_gemm_kernel<2>", "pw_wgrad_kernel<128, 2>"),
+         "136 channels both ways: every op on shifted copies"),
     # ---- 1x1: pw_gemm_kernel<MB>, pw_wgrad_kernel<NBLK, MG>
     Case(13, 13, 1, 1, 1, 2, 8, 24, True, K("pw_gemm_kernel<1>", "pw_wgrad_kernel<16, 1>"),
          "P = 192: last 128-pixel tile partial"),
@@ -173,6 +184,12 @@ def table_instances():
     for c in CASES:
         out |= c.launches
     return out | FIXUP_FWD | FIXUP_WGRAD
+
+
+def shifted_copy_only(c):
+    """stride-1 multi-tap rows with more than 128 channels on both sides: conv_tap_kernel and wgrad_tap_kernel take at
+    most 128, so fprop, dgrad and wgrad all run on pw_gemm_kernel / pw_wgrad_kernel (over shifted copies when S > 1)"""
+    return c.stride == 1 and c.R * c.S > 1 and min(c.C, c.K) > 128
 
 
 def case_id(c):
@@ -420,6 +437,8 @@ def test_case_against_fp64(c):
     kf, kd, kw, (d, x, strips, dy, w, ref, A, retrace) = run_and_check(c, [0] * 9, case_id(c))
     assert launched(kf | kd | kw, lambda k: c.launches <= k, retrace), \
         "%s did not launch %s (launched: %s)" % (case_id(c), sorted(c.launches - (kf | kd | kw)), sorted(kf | kd | kw))
+    if shifted_copy_only(c):
+        assert not {"conv_tap_kernel", "wgrad_tap_kernel"} & _names(kf | kd | kw), sorted(kf | kd | kw)
     # accumulate=1 adds onto what dw / db hold
     g = torch.Generator(device=DEV).manual_seed(7)
     dw0 = torch.randn(w.shape, generator=g, device=DEV) * float(ref["dw"].abs().mean())
@@ -523,26 +542,6 @@ def test_halo_masks(c, grid, path):
             k, retrace = run_boundary_direct(c, mask, tag, *DIRECT_PATHS[path])
             assert launched(k, lambda k: "conv_direct_kernel" in _names(k), retrace) == fix, (tag, fix, sorted(k))
             assert "halo_im2col_kernel" not in _names(k), (tag, sorted(k))
-
-
-TAP_CASES = [c for c in CASES if c.stride == 1 and c.R * c.S > 1]
-
-
-@pytest.mark.parametrize("c", TAP_CASES, ids=case_id)
-def test_case_shifted_copy_path(c, monkeypatch):
-    """SPC_TAP_V1=1: the stride-1 multi-tap layers on column-shifted HBM copies + pw_gemm / pw_wgrad"""
-    L = _lib.lib()
-    monkeypatch.setenv("SPC_TAP_V1", "1")
-    L.spc_reload_env()
-    try:
-        kf, kd, kw, rest = run_and_check(c, [0] * 9, case_id(c) + " tap_v1")
-        k = kf | kd | kw
-        assert not {"conv_tap_kernel", "wgrad_tap_kernel"} & _names(k), sorted(k)
-        want = {"pw_gemm_kernel", "pw_wgrad_kernel"} | ({"shift_copies_vec_kernel"} if c.S > 1 else set())
-        assert launched(k, lambda k: want <= _names(k), rest[-1]), (sorted(want), sorted(k))
-    finally:
-        monkeypatch.delenv("SPC_TAP_V1")
-        L.spc_reload_env()
 
 
 def test_wgrad_empty_batch_accumulate():
