@@ -40,7 +40,8 @@ def get_parser(exchange_only_default=False):
     p.add_argument("--enable-val-conv", action="store_true", default=False, help="Enable validation of convolution")
     p.add_argument("--enable-val-small-conv", action="store_true", default=False,
                    help="accepted for compatibility: the convolution here is deterministic, --enable-val-conv covers it")
-    p.add_argument("--enable-deterministic", action="store_true", default=False, help="accepted for compatibility")
+    p.add_argument("--enable-deterministic", action="store_true", default=False,
+                   help="torch.use_deterministic_algorithms(True): bit-reproducible weight gradients")
     p.add_argument("--enable-one-h-dim-kernel", action="store_true", default=False, help="Set dimension (height) of kernel to 1")
     p.add_argument("--enable-one-w-dim-kernel", action="store_true", default=False, help="Set dimension (width) of kernel to 1")
     p.add_argument("--num-spatial-parts", type=int, default=4, help="Number of partitions in spatial parallelism")
@@ -53,6 +54,8 @@ def get_parser(exchange_only_default=False):
 
 def main(exchange_only_default=False):
     args = get_parser(exchange_only_default).parse_args()
+    if args.enable_deterministic:
+        torch.use_deterministic_algorithms(True)
     gems_comm.initialize_cuda()
     if not dist.is_initialized():
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")

@@ -29,14 +29,25 @@ from mpi4dl_b200.torchgems.train_spatial import get_shapes_spatial, split_input 
 from mpi4dl_b200.torchgems.train_spatial_master import train_spatial_model_master, verify_spatial_master_config  # noqa: E402
 
 
-def main(kind):
+def get_parser():
     p = parser.get_parser()
     p.add_argument("--dtype", choices=["fp32", "bf16", "bf16-amp"], default="fp32",
                    help="bf16-amp: fp32 parameters, the forward under torch.autocast(dtype=torch.bfloat16)")
     p.add_argument("--recompute", action="store_true",
                    help="keep only each spatial cell's input and halo strips for backward and recompute the cell there")
+    p.add_argument("--deterministic", action="store_true",
+                   help="torch.use_deterministic_algorithms(True): bit-reproducible steps, the convolution weight "
+                        "gradients included")
     p.add_argument("--steps", type=int, default=10)
-    args = p.parse_args()
+    return p
+
+
+def main(kind):
+    args = get_parser().parse_args()
+    if args.deterministic:
+        # before CUDA initialises: cuBLAS (the nn.Linear of the pipeline's tail) needs it in deterministic mode
+        os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
+        torch.use_deterministic_algorithms(True)
     gems_comm.initialize_cuda()
     np.random.seed(seed=1405)
     batch_size, parts, image_size = args.batch_size, args.parts, int(args.image_size)

@@ -11,7 +11,8 @@ Same command line as the reference's benchmarks/spatial_parallelism/benchmark_{r
 world size = spatial_size * P + split_size - spatial_size.  Extra flags of this script: --dtype
 {fp32,bf16,bf16-amp} (bf16 puts the spatial convs on the wgmma kernels; bf16-amp too, with fp32
 master weights under torch.autocast), --recompute (recompute the spatial cells in backward from their
-inputs and recorded halo strips), --steps N (synthetic batches per epoch, default 10).  APP 3 (synthetic) needs no dataset; APP 1/2 use torchvision like the reference.
+inputs and recorded halo strips), --deterministic (torch.use_deterministic_algorithms(True): bit-reproducible
+steps), --steps N (synthetic batches per epoch, default 10).  APP 3 (synthetic) needs no dataset; APP 1/2 use torchvision like the reference.
 """
 import math
 import os
@@ -84,14 +85,25 @@ def _batches(args, image_size, batch_size, steps):
     yield from dl
 
 
-def main(kind):
+def get_parser():
     p = parser.get_parser()
     p.add_argument("--dtype", choices=["fp32", "bf16", "bf16-amp"], default="fp32",
                    help="bf16-amp: fp32 parameters, the forward under torch.autocast(dtype=torch.bfloat16)")
     p.add_argument("--recompute", action="store_true",
                    help="keep only each spatial cell's input and halo strips for backward and recompute the cell there")
+    p.add_argument("--deterministic", action="store_true",
+                   help="torch.use_deterministic_algorithms(True): bit-reproducible steps, the convolution weight "
+                        "gradients included")
     p.add_argument("--steps", type=int, default=10)
-    args = p.parse_args()
+    return p
+
+
+def main(kind):
+    args = get_parser().parse_args()
+    if args.deterministic:
+        # before CUDA initialises: cuBLAS (the nn.Linear of the pipeline's tail) needs it in deterministic mode
+        os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
+        torch.use_deterministic_algorithms(True)
     gems_comm.initialize_cuda()
     np.random.seed(seed=1405)
 

@@ -126,7 +126,24 @@ int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo
                      float* dw, float* db, int accumulate, void* workspace,
                      size_t workspace_bytes, void* stream);
 
-size_t spc_conv_workspace_bytes(const spc_conv_desc* d, int op /*0 fwd, 1 dgrad, 2 wgrad*/);
+/* spc_conv2d_wgrad with bit-reproducible results: the same arguments, and dw / db are bit-identical whenever x, the
+ * strips, dy and (accumulate != 0) the initial dw / db are, on GPUs with the same SM count.  The default wgrad adds its
+ * partial sums into dw with fp32 atomics in whatever order the CTAs finish; this one gives each slice of the work (a
+ * pixel-range split, an image strip, a CTA column, a bias chunk: units whose adds never meet on one element) a zeroed
+ * copy in the workspace and sums the copies into dw in slice order, the halo strips' share after the tile's.  Each
+ * element gets as many fp32 roundings as with spc_conv2d_wgrad, so the per-element error bounds stated above for each
+ * path (bf16, TF32 1x1 / tap / stride-2, direct) hold unchanged; the bits may differ from spc_conv2d_wgrad's.
+ * workspace: spc_conv_workspace_bytes(d, 3) bytes, non-zero on every path.  It exceeds op 2's by at most
+ * SPC_WGRAD_SLICE_BYTES_MAX; launches with more slices than fit run in passes, with the same bits.  A smaller workspace,
+ * down to op 2's size, is accepted and gives the same bits in more passes.
+ * torchgems calls this instead of spc_conv2d_wgrad when torch.are_deterministic_algorithms_enabled(). */
+#define SPC_WGRAD_SLICE_BYTES_MAX ((size_t)256 << 20)
+int spc_conv2d_wgrad_deterministic(const spc_conv_desc* d, const void* x, const spc_halo* halo, const void* dy,
+                                   float* dw, float* db, int accumulate, void* workspace,
+                                   size_t workspace_bytes, void* stream);
+
+size_t spc_conv_workspace_bytes(const spc_conv_desc* d,
+                                int op /*0 fwd, 1 dgrad, 2 wgrad, 3 spc_conv2d_wgrad_deterministic*/);
 /* 1 if the tensor-core (wgmma) kernel will be used for this op, else 0 (direct kernel); the name is historical */
 int    spc_conv_uses_tcgen05(const spc_conv_desc* d, int op);
 /* output extent of a tile: Ho = (H + 2*pad_h - R)/stride_h + 1 */

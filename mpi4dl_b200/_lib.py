@@ -37,6 +37,8 @@ SYMBOLS = [
     ("spc_conv2d_fwd_boundary", C.c_int, [C.POINTER(ConvDesc), _P, C.POINTER(Halo), _P, _P, _P, _P]),
     ("spc_conv2d_dgrad", C.c_int, [C.POINTER(ConvDesc), _P, _P, _P, _P, C.c_size_t, _P]),
     ("spc_conv2d_wgrad", C.c_int, [C.POINTER(ConvDesc), _P, C.POINTER(Halo), _P, _P, _P, C.c_int, _P, C.c_size_t, _P]),
+    ("spc_conv2d_wgrad_deterministic", C.c_int,
+     [C.POINTER(ConvDesc), _P, C.POINTER(Halo), _P, _P, _P, C.c_int, _P, C.c_size_t, _P]),
     ("spc_conv_workspace_bytes", C.c_size_t, [C.POINTER(ConvDesc), C.c_int]),
     ("spc_conv_uses_tcgen05", C.c_int, [C.POINTER(ConvDesc), C.c_int]),
     ("spc_conv_out_shape", None, [C.POINTER(ConvDesc), C.POINTER(C.c_int), C.POINTER(C.c_int)]),

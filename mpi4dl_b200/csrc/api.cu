@@ -112,7 +112,8 @@ static int boundary_fwd_tc(const spc_conv_desc* d, const void* x, const spc_halo
   return launch_boundary_scatter(O, b, d->K, Ho, Wo, y, st);
 }
 
-static int boundary_wgrad_tc(const spc_conv_desc* d, const spc_halo* halo, const void* dy, float* dw, cudaStream_t st) {
+static int boundary_wgrad_tc(const spc_conv_desc* d, const spc_halo* halo, const void* dy, float* dw, cudaStream_t st,
+                             const WgradSlices* sl) {
   int Ho, Wo;
   spc_conv_out_shape(d, &Ho, &Wo);
   BoundaryRects b;
@@ -127,7 +128,7 @@ static int boundary_wgrad_tc(const spc_conv_desc* d, const spc_halo* halo, const
   if (rc) return rc;
   rc = launch_boundary_gather(dy, b, d->K, Ho, Wo, G, st);
   if (rc) return rc;
-  return tc_pw_wgrad(V, G, dw, d->K, CT, b.padded, st);   // dw[k][(c,r,s)] += sum_p G[k][p] * V[(c,r,s)][p]
+  return tc_pw_wgrad(V, G, dw, d->K, CT, b.padded, st, sl);   // dw[k][(c,r,s)] += sum_p G[k][p] * V[(c,r,s)][p]
 }
 
 // Launch the direct kernel on the output sub-rectangle [y0,y1) x [x0,x1).
@@ -169,8 +170,38 @@ int spc_conv_uses_tcgen05(const spc_conv_desc* d, int op) {
 static bool tf32_pointwise(const spc_conv_desc* d) { return d->R == 1 && d->S == 1; }
 static bool tf32_strided(const spc_conv_desc* d) { return d->stride_h == 2; }
 
+// Slice copies of the deterministic wgrad: the most slices one launch of this shape's wgrad can have, times the
+// gradient's size, capped at SPC_WGRAD_SLICE_BYTES_MAX (larger launches run in passes, with the same bits):
+//   wgmma / TF32 1x1 kernels: splits <= 2 * SMs / groups and dw <= groups * 128 x 256 elements, so <= 2 * SMs * 32768;
+//   bf16 tap kernel: <= 3 waves of items, or one slice per (image, strip) when those alone fill more;
+//   TF32 tap kernels: >= chunks / 512 splits (the longest chain an item may sum), else <= 2 * SMs;
+//   direct kernel: its CTA columns;  bias: <= 64 chunks of K.
+static size_t wgrad_slice_bytes(const spc_conv_desc* d) {
+  int Ho, Wo;
+  spc_conv_out_shape(d, &Ho, &Wo);
+  const double wn = (double)d->K * d->C * d->R * d->S, sms = tc_sm_count();
+  const double pw = 2.0 * sms * (wn < 32768.0 ? wn : 32768.0);
+  const auto direct = [&](int rH, int rW) { return (double)wgrad_direct_slices(d->N, d->K, d->C, rH, rW) * wn; };
+  double need = 64.0 * d->K;
+  const bool tc = spc_conv_uses_tcgen05(d, 2);
+  if (!tc) {
+    need = fmax(need, direct(Ho, Wo));
+  } else if (d->dtype == SPC_BF16) {
+    const double tap = fmax(3.0 * sms, (double)d->N * (d->W / 64)) * wn;
+    need = fmax(need, d->R * d->S > 1 && d->stride_h == 1 && d->W % 64 == 0 ? fmax(tap, pw) : pw);
+  } else if (d->R * d->S == 1) {
+    need = fmax(need, pw);
+  } else {
+    const double chunks = (double)d->N * Ho * ((Wo + 31) / 32);
+    need = fmax(need, fmax(2.0 * sms, ceil(chunks / 512.0)) * wn);
+    need = fmax(need, fmax(direct(Ho, d->pad_w), direct(d->pad_h, Wo)));   // the boundary rectangles' share
+  }
+  return (size_t)fmin(need * sizeof(float), (double)SPC_WGRAD_SLICE_BYTES_MAX);
+}
+
 size_t spc_conv_workspace_bytes(const spc_conv_desc* d, int op) {
   if (!d) return 0;
+  if (op == 3) return validate(d) ? 0 : al256(spc_conv_workspace_bytes(d, 2)) + al256(wgrad_slice_bytes(d));
   if (!spc_conv_uses_tcgen05(d, op)) return 0;
   if (d->dtype == SPC_BF16) return tc_workspace_bytes(d, op);
   if (tf32_pointwise(d)) return tf32_workspace_bytes(d, op);
@@ -298,12 +329,10 @@ int spc_conv2d_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void
   return SPC_OK;
 }
 
-int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo, const void* dy, float* dw,
-                     float* db, int accumulate, void* workspace, size_t workspace_bytes, void* stream) {
-  int rc = validate(d);
-  if (rc) return rc;
-  SPC_REQUIRE(dw && (d->N == 0 || (x && dy)), "conv_wgrad: null tensor pointer");
-  cudaStream_t st = (cudaStream_t)stream;
+// sl == nullptr: every kernel adds straight into dw / db; else through slice copies summed in order (common.cuh)
+static int wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo, const void* dy, float* dw, float* db,
+                 int accumulate, void* workspace, size_t workspace_bytes, cudaStream_t st, const WgradSlices* sl) {
+  int rc = SPC_OK;
   int Ho, Wo;
   spc_conv_out_shape(d, &Ho, &Wo);
   const size_t wn = (size_t)d->K * d->C * d->R * d->S;
@@ -319,10 +348,10 @@ int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo
   }
   if (tc && d->dtype == SPC_F32 && tf32_pointwise(d)) {
     // 1x1: no output window reaches a halo strip, so there is nothing to add for the strips
-    rc = tf32_conv_wgrad(d, x, dy, dw, workspace, workspace_bytes, st);
+    rc = tf32_conv_wgrad(d, x, dy, dw, workspace, workspace_bytes, st, sl);
     if (rc) return rc;
   } else if (tc && d->dtype == SPC_F32) {
-    rc = tf32_strided(d) ? tf32_tap_s2_wgrad(d, x, dy, dw, st) : tf32_tap_wgrad(d, x, dy, dw, st);
+    rc = tf32_strided(d) ? tf32_tap_s2_wgrad(d, x, dy, dw, st, sl) : tf32_tap_wgrad(d, x, dy, dw, st, sl);
     if (rc) return rc;
     // the halo pixels' share (exact by linearity): the direct kernel over the outputs whose windows reach a strip,
     // reading the strips through the halo-only view (zero inside the tile)
@@ -335,16 +364,16 @@ int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo
         q.K = d->K; q.R = d->R; q.S = d->S; q.sh = d->stride_h; q.sw = d->stride_w; q.ph = d->pad_h; q.pw = d->pad_w;
         q.Ho = Ho; q.Wo = Wo;
         q.ry0 = b.y0[i]; q.rx0 = b.x0[i]; q.rH = b.y1[i] - b.y0[i]; q.rW = b.x1[i] - b.x0[i];
-        rc = launch_wgrad_direct(q, SPC_F32, st);
+        rc = launch_wgrad_direct(q, SPC_F32, st, sl);
         if (rc) return rc;
       }
     }
   } else if (tc) {
-    rc = tc_conv_wgrad(d, x, dy, dw, workspace, workspace_bytes, st);
+    rc = tc_conv_wgrad(d, x, dy, dw, workspace, workspace_bytes, st, sl);
     if (rc) return rc;
     // add the halo pixels' contribution (exact by linearity): boundary GEMM over the outputs whose windows reach a strip
     if (has_halo(halo)) {
-      rc = boundary_wgrad_tc(d, halo, dy, dw, st);
+      rc = boundary_wgrad_tc(d, halo, dy, dw, st, sl);
       if (rc) return rc;
     }
   } else {
@@ -353,11 +382,37 @@ int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo
     p.dy = dy; p.dw = dw;
     p.K = d->K; p.R = d->R; p.S = d->S; p.sh = d->stride_h; p.sw = d->stride_w; p.ph = d->pad_h; p.pw = d->pad_w;
     p.Ho = Ho; p.Wo = Wo;
-    rc = launch_wgrad_direct(p, d->dtype, st);
+    rc = launch_wgrad_direct(p, d->dtype, st, sl);
     if (rc) return rc;
   }
-  if (db) return launch_bias_grad(dy, db, d->N, d->K, Ho * Wo, d->dtype, accumulate, st);
+  if (db) return launch_bias_grad(dy, db, d->N, d->K, Ho * Wo, d->dtype, accumulate, st, sl);
   return SPC_OK;
+}
+
+int spc_conv2d_wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo, const void* dy, float* dw,
+                     float* db, int accumulate, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = validate(d);
+  if (rc) return rc;
+  SPC_REQUIRE(dw && (d->N == 0 || (x && dy)), "conv_wgrad: null tensor pointer");
+  return wgrad(d, x, halo, dy, dw, db, accumulate, workspace, workspace_bytes, (cudaStream_t)stream, nullptr);
+}
+
+int spc_conv2d_wgrad_deterministic(const spc_conv_desc* d, const void* x, const spc_halo* halo, const void* dy, float* dw,
+                                   float* db, int accumulate, void* workspace, size_t workspace_bytes, void* stream) {
+  int rc = validate(d);
+  if (rc) return rc;
+  SPC_REQUIRE(dw && (d->N == 0 || (x && dy)), "conv_wgrad_deterministic: null tensor pointer");
+  // [0, op 2's workspace): the kernels' own operands; the rest holds slice copies.  Less than op 3's size still works,
+  // in more passes with the same bits; none at all adds one slice per launch straight into dw.
+  const size_t own = al256(spc_conv_workspace_bytes(d, 2));
+  SPC_REQUIRE(workspace_bytes >= own && (own == 0 || workspace),
+              "conv_wgrad_deterministic: workspace of %zu bytes, need at least %zu", workspace_bytes, own);
+  WgradSlices sl{nullptr, 0};
+  if (workspace && workspace_bytes > own) {
+    sl.buf = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + own);
+    sl.elems = (workspace_bytes - own) / sizeof(float);
+  }
+  return wgrad(d, x, halo, dy, dw, db, accumulate, workspace, workspace_bytes, (cudaStream_t)stream, &sl);
 }
 
 }  // extern "C"

@@ -116,6 +116,43 @@ inline TileView make_view(const void* x, const spc_halo* halo, int N, int C, int
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 inline size_t dtype_size(int dt) { return dt == SPC_BF16 ? 2 : 4; }
 
+// ---- deterministic wgrad (spc_conv2d_wgrad_deterministic): wgrad_reduce.cu ------------------------------------------
+// Every wgrad kernel flushes its partial sums with fp32 atomics.  Its work is cut into slices (a pixel-range split, an
+// (image, strip, row range), a CTA column, a bias chunk) within which no two adds land on the same element of dw.  A
+// launch covers slices [split0, split0 + nsplit) and adds slice s into dw + (s - split0) * slice_stride.  The default
+// path launches all slices with stride 0: everything lands in dw, in the order the CTAs finish.  The deterministic path
+// gives each slice its own zeroed copy (0 + v == v exactly) and sums the copies into dw in slice order.
+struct WgradSlices {
+  float* buf;      // slice copies, 256-byte aligned
+  size_t elems;    // capacity in floats
+};
+// dw[i] = (((dw[i] + buf[0][i]) + buf[1][i]) + ... + buf[n-1][i]), buf[j] = buf + j * wn
+int reduce_slices(float* dw, const float* buf, int n, size_t wn, cudaStream_t st);
+// Run launch(split0, nsplit, dst, slice_stride) over slices [0, slices) of a gradient of wn floats at dw.  sl == nullptr:
+// one launch of every slice straight into dw.  Otherwise passes of as many slices as sl->buf holds, each summed into dw
+// before the next; a pass of one slice adds straight into dw.  The sum is one left-to-right chain, so the bits do not
+// depend on the pass size.
+template <class Launch>
+int run_slices(const WgradSlices* sl, int slices, size_t wn, float* dw, cudaStream_t st, Launch&& launch) {
+  if (!sl) return launch(0, slices, dw, (size_t)0);
+  const size_t fit = wn ? sl->elems / wn : 0;
+  const int per = fit >= (size_t)slices ? slices : (int)(fit > 0 ? fit : 1);
+  for (int s0 = 0; s0 < slices; s0 += per) {
+    const int n = slices - s0 < per ? slices - s0 : per;
+    if (n == 1) {
+      const int rc = launch(s0, 1, dw, (size_t)0);
+      if (rc) return rc;
+      continue;
+    }
+    SPC_CHECK_CUDA(cudaMemsetAsync(sl->buf, 0, (size_t)n * wn * sizeof(float), st));
+    int rc = launch(s0, n, sl->buf, wn);
+    if (rc) return rc;
+    rc = reduce_slices(dw, sl->buf, n, wn, st);
+    if (rc) return rc;
+  }
+  return SPC_OK;
+}
+
 // ---- direct (CUDA-core) kernels: conv_direct.cu ----------------------------------------
 // Generalised correlation: y[n,k, oy0+i*oys, ox0+j*oxs] = bias[k] + sum_{c,r,s}
 //   w[w_off + k*wKs + c*wCs + r*wRs + s*wSs] * in(n, c, i*sh + r - pt, j*sw + s - pl)
@@ -140,9 +177,14 @@ struct DirectWgradParams {
   float* dw;          // [K][C][R][S] fp32, accumulated with atomics (zeroed by caller)
   int K, R, S, sh, sw, ph, pw, Ho, Wo;
   int ry0, rx0, rH, rW;   // output sub-rectangle to reduce over (rH == 0: the whole output)
+  int split0;             // slice (CTA column) of blockIdx.x == 0; slice s adds into dw + (s - split0) * slice_stride
+  size_t slice_stride;
 };
-int launch_wgrad_direct(const DirectWgradParams& p, int dtype, cudaStream_t st);
-int launch_bias_grad(const void* dy, float* db, int N, int K, int HW, int dtype, int accumulate, cudaStream_t st);
+int launch_wgrad_direct(const DirectWgradParams& p, int dtype, cudaStream_t st, const WgradSlices* sl = nullptr);
+int launch_bias_grad(const void* dy, float* db, int N, int K, int HW, int dtype, int accumulate, cudaStream_t st,
+                     const WgradSlices* sl = nullptr);
+// CTA columns (slices) of launch_wgrad_direct over an output rectangle of rH x rW; 0 if empty
+int wgrad_direct_slices(int N, int K, int C, int rH, int rW);
 
 // ---- halo fix-up as a small GEMM over the boundary outputs only (halo.cu kernels, api.cu orchestration) ----------
 void* boundary_scratch(size_t bytes);   // grow-only device scratch of the fix-up's operands
@@ -165,7 +207,8 @@ int launch_boundary_scatter(const void* O, const BoundaryRects& b, int K, int Ho
 size_t tc_pw_workspace_bytes(int M, int Cin);
 int tc_pw_fwd(const void* w, int ld, int M, int Cin, const void* x, const void* bias, void* y, int P, void* ws, size_t ws_bytes,
               cudaStream_t st);
-int tc_pw_wgrad(const void* x, const void* dy, float* dw, int K, int C, int P, cudaStream_t st);
+int tc_pw_wgrad(const void* x, const void* dy, float* dw, int K, int C, int P, cudaStream_t st,
+                const WgradSlices* sl = nullptr);
 
 // ---- wgmma pointwise GEMM path: gemm_tc.cu -----------------------------------------------
 bool tc_supported(const spc_conv_desc* d, int op);
@@ -175,7 +218,8 @@ int tc_conv_fwd(const spc_conv_desc* d, const void* x, const void* w, const void
 int tc_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* dx, void* ws,
                   size_t ws_bytes, cudaStream_t st);
 int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void* ws,
-                  size_t ws_bytes, cudaStream_t st);
+                  size_t ws_bytes, cudaStream_t st, const WgradSlices* sl = nullptr);
+int tc_sm_count();
 
 // ---- fp32 1x1 convolutions on TF32 wgmma (SPC_ALGO_TF32): gemm_tf32.cu ---------------------------------------------
 bool tf32_supported(const spc_conv_desc* d);
@@ -185,7 +229,7 @@ int tf32_conv_fwd(const spc_conv_desc* d, const void* x, const void* w, const vo
 int tf32_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* dx, void* ws, size_t ws_bytes,
                     cudaStream_t st);
 int tf32_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void* ws, size_t ws_bytes,
-                    cudaStream_t st);
+                    cudaStream_t st, const WgradSlices* sl = nullptr);
 
 // ---- fp32 stride-1 multi-tap convolutions on TF32 wgmma (SPC_ALGO_TF32_ALL): conv_tap_tf32.cu ----------------------
 bool tf32_tap_supported(const spc_conv_desc* d);
@@ -195,7 +239,8 @@ int tf32_tap_fwd(const spc_conv_desc* d, const void* x, const void* w, const voi
 int tf32_tap_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* dx, void* ws, size_t ws_bytes,
                    cudaStream_t st);
 // the interior's share of dw (zero padding), added with atomics; api.cu adds the halo strips' share
-int tf32_tap_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st);
+int tf32_tap_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st,
+                   const WgradSlices* sl = nullptr);
 
 // ---- fp32 stride-2 multi-tap convolutions on TF32 wgmma (SPC_ALGO_TF32_STRIDED): conv_tap_s2_tf32.cu ---------------
 bool tf32_tap_s2_supported(const spc_conv_desc* d);
@@ -205,6 +250,7 @@ int tf32_tap_s2_fwd(const spc_conv_desc* d, const void* x, const void* w, const 
 int tf32_tap_s2_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* dx, void* ws, size_t ws_bytes,
                       cudaStream_t st);
 // the interior's share of dw (zero padding), added with atomics; api.cu adds the halo strips' share
-int tf32_tap_s2_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st);
+int tf32_tap_s2_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st,
+                      const WgradSlices* sl = nullptr);
 
 }  // namespace spc

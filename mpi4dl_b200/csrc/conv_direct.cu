@@ -163,7 +163,7 @@ wgrad_direct_kernel(const DirectWgradParams p, const int kblocks, const int cblo
   const int kl = threadIdx.x / WG_CB, cl = threadIdx.x % WG_CB;
   const int C = p.in.C;
   const int total_tiles = p.in.N * tiles_x * tiles_y;
-  const int t_begin = blockIdx.x * tiles_per_cta;
+  const int t_begin = (blockIdx.x + p.split0) * tiles_per_cta;
   const int t_end = min(total_tiles, t_begin + tiles_per_cta);
 
   float acc[WG_TAPS];
@@ -213,18 +213,20 @@ wgrad_direct_kernel(const DirectWgradParams p, const int kblocks, const int cblo
     }
   }
   if (k0 + kl < p.K && c0 + cl < C) {
+    float* dw = p.dw + blockIdx.x * p.slice_stride;
 #pragma unroll
     for (int t = 0; t < WG_TAPS; ++t) {
-      if (t < ntaps) atomicAdd(&p.dw[((size_t)(k0 + kl) * C + (c0 + cl)) * (p.R * p.S) + tap0 + t], acc[t]);
+      if (t < ntaps) atomicAdd(&dw[((size_t)(k0 + kl) * C + (c0 + cl)) * (p.R * p.S) + tap0 + t], acc[t]);
     }
   }
 }
 
+// slice = chunk: chunk split0 + blockIdx.y adds into db + blockIdx.y * slice_stride
 template <typename T>
 __global__ void bias_grad_kernel(const T* __restrict__ dy, float* __restrict__ db, int N, int K, int HW,
-                                 int chunks) {
+                                 int chunks, int split0, size_t slice_stride) {
   const int k = blockIdx.x;
-  const int chunk = blockIdx.y;
+  const int chunk = blockIdx.y + split0;
   float s = 0.f;
   for (int n = 0; n < N; ++n) {
     const T* base = dy + ((size_t)n * K + k) * HW;
@@ -239,7 +241,7 @@ __global__ void bias_grad_kernel(const T* __restrict__ dy, float* __restrict__ d
   if (threadIdx.x < 32) {
     s = (threadIdx.x < (blockDim.x >> 5)) ? red[threadIdx.x] : 0.f;
     for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if (threadIdx.x == 0) atomicAdd(&db[k], s);
+    if (threadIdx.x == 0) atomicAdd(&db[blockIdx.y * slice_stride + k], s);
   }
 }
 
@@ -289,7 +291,22 @@ int launch_conv_direct(const DirectConvParams& p, int dtype, cudaStream_t st) {
   return SPC_OK;
 }
 
-int launch_wgrad_direct(const DirectWgradParams& p_in, int dtype, cudaStream_t st) {
+// enough CTAs for ~4 waves of 132 SMs x 2 resident CTAs, but at least 8 tiles each
+static int direct_tiles_per_cta(int N, int K, int C, int rH, int rW) {
+  const int total_tiles = N * ceil_div(rW, WG_TW) * ceil_div(rH, WG_TH);
+  int want = (132 * 8) / (ceil_div(K, WG_KB) * ceil_div(C, WG_CB));
+  if (want < 1) want = 1;
+  int tiles_per_cta = ceil_div(total_tiles, want);
+  if (tiles_per_cta < 8) tiles_per_cta = 8;
+  return tiles_per_cta;
+}
+
+int wgrad_direct_slices(int N, int K, int C, int rH, int rW) {
+  if (rH <= 0 || rW <= 0 || N <= 0) return 0;
+  return ceil_div(N * ceil_div(rW, WG_TW) * ceil_div(rH, WG_TH), direct_tiles_per_cta(N, K, C, rH, rW));
+}
+
+int launch_wgrad_direct(const DirectWgradParams& p_in, int dtype, cudaStream_t st, const WgradSlices* sl) {
   DirectWgradParams p = p_in;
   if (p.rH == 0 && p.rW == 0) { p.ry0 = 0; p.rx0 = 0; p.rH = p.Ho; p.rW = p.Wo; }
   if (p.rH <= 0 || p.rW <= 0 || p.in.N <= 0) return SPC_OK;
@@ -299,54 +316,60 @@ int launch_wgrad_direct(const DirectWgradParams& p_in, int dtype, cudaStream_t s
   SPC_REQUIRE(smem <= 200 * 1024, "wgrad_direct: filter %dx%d needs %zu B smem", p.R, p.S, smem);
   const int tiles_x = ceil_div(p.rW, WG_TW), tiles_y = ceil_div(p.rH, WG_TH);
   const int kblocks = ceil_div(p.K, WG_KB), cblocks = ceil_div(p.in.C, WG_CB);
-  const int total_tiles = p.in.N * tiles_x * tiles_y;
-  // enough CTAs for ~4 waves of 132 SMs x 2 resident CTAs, but at least 8 tiles each
-  int want = (132 * 8) / (kblocks * cblocks);
-  if (want < 1) want = 1;
-  int tiles_per_cta = ceil_div(total_tiles, want);
-  if (tiles_per_cta < 8) tiles_per_cta = 8;
-  const int ctas_x = ceil_div(total_tiles, tiles_per_cta);
-  dim3 grid(ctas_x, kblocks * cblocks);
+  const int tiles_per_cta = direct_tiles_per_cta(p.in.N, p.K, p.in.C, p.rH, p.rW);
+  const int ctas_x = wgrad_direct_slices(p.in.N, p.K, p.in.C, p.rH, p.rW);
   const int taps = p.R * p.S;
-  for (int tap0 = 0; tap0 < taps; tap0 += WG_TAPS) {
-    const int nt = taps - tap0 < WG_TAPS ? taps - tap0 : WG_TAPS;
-    if (dtype == SPC_BF16) {
-      static bool attr_bf16 = false;
-      if (!attr_bf16) {
-        SPC_CHECK_CUDA(cudaFuncSetAttribute(wgrad_direct_kernel<__nv_bfloat16>,
-                                            cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-        attr_bf16 = true;
+  const size_t wn = (size_t)p.K * p.in.C * taps;
+  // slice = CTA column: its tiles are summed in registers, its adds cover disjoint (k, c) blocks
+  return run_slices(sl, ctas_x, wn, p.dw, st, [&](int s0, int ns, float* dst, size_t stride) {
+    DirectWgradParams q = p;
+    q.split0 = s0; q.dw = dst; q.slice_stride = stride;
+    dim3 grid(ns, kblocks * cblocks);
+    for (int tap0 = 0; tap0 < taps; tap0 += WG_TAPS) {
+      const int nt = taps - tap0 < WG_TAPS ? taps - tap0 : WG_TAPS;
+      if (dtype == SPC_BF16) {
+        static bool attr_bf16 = false;
+        if (!attr_bf16) {
+          SPC_CHECK_CUDA(cudaFuncSetAttribute(wgrad_direct_kernel<__nv_bfloat16>,
+                                              cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+          attr_bf16 = true;
+        }
+        wgrad_direct_kernel<__nv_bfloat16><<<grid, WG_THREADS, smem, st>>>(q, kblocks, cblocks, tiles_x, tiles_y,
+                                                                           tiles_per_cta, tap0, nt);
+      } else {
+        static bool attr_f32 = false;
+        if (!attr_f32) {
+          SPC_CHECK_CUDA(cudaFuncSetAttribute(wgrad_direct_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              200 * 1024));
+          attr_f32 = true;
+        }
+        wgrad_direct_kernel<float><<<grid, WG_THREADS, smem, st>>>(q, kblocks, cblocks, tiles_x, tiles_y,
+                                                                  tiles_per_cta, tap0, nt);
       }
-      wgrad_direct_kernel<__nv_bfloat16><<<grid, WG_THREADS, smem, st>>>(p, kblocks, cblocks, tiles_x, tiles_y,
-                                                                         tiles_per_cta, tap0, nt);
-    } else {
-      static bool attr_f32 = false;
-      if (!attr_f32) {
-        SPC_CHECK_CUDA(cudaFuncSetAttribute(wgrad_direct_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            200 * 1024));
-        attr_f32 = true;
-      }
-      wgrad_direct_kernel<float><<<grid, WG_THREADS, smem, st>>>(p, kblocks, cblocks, tiles_x, tiles_y,
-                                                                tiles_per_cta, tap0, nt);
+      spc::count_launch();
+      SPC_CHECK_CUDA(cudaGetLastError());
     }
-    spc::count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  }
-  return SPC_OK;
+    return SPC_OK;
+  });
 }
 
-int launch_bias_grad(const void* dy, float* db, int N, int K, int HW, int dtype, int accumulate, cudaStream_t st) {
+int launch_bias_grad(const void* dy, float* db, int N, int K, int HW, int dtype, int accumulate, cudaStream_t st,
+                     const WgradSlices* sl) {
   if (!accumulate) SPC_CHECK_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * K, st));
   int chunks = ceil_div(HW, 1 << 16);
   if (chunks > 64) chunks = 64;
-  dim3 grid(K, chunks);
-  if (dtype == SPC_BF16)
-    bias_grad_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(dy), db, N, K, HW, chunks);
-  else
-    bias_grad_kernel<float><<<grid, 256, 0, st>>>(reinterpret_cast<const float*>(dy), db, N, K, HW, chunks);
-  spc::count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  return SPC_OK;
+  return run_slices(sl, chunks, (size_t)K, db, st, [&](int s0, int ns, float* dst, size_t stride) {
+    dim3 grid(K, ns);
+    if (dtype == SPC_BF16)
+      bias_grad_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(dy), dst, N, K, HW,
+                                                            chunks, s0, stride);
+    else
+      bias_grad_kernel<float><<<grid, 256, 0, st>>>(reinterpret_cast<const float*>(dy), dst, N, K, HW, chunks, s0,
+                                                    stride);
+    spc::count_launch();
+    SPC_CHECK_CUDA(cudaGetLastError());
+    return SPC_OK;
+  });
 }
 
 }  // namespace spc

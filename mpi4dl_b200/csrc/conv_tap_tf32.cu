@@ -355,6 +355,8 @@ struct TapWgParams {
   int splits;            // row-segment ranges per (tap, channel block, output group)
   int chunks_total;      // N * H * segs_row
   int stages;
+  int split0, nsplit;    // this launch runs splits [split0, split0 + nsplit)
+  size_t slice_stride;   // split sp adds into dw + (sp - split0) * slice_stride (common.cuh: WgradSlices)
 };
 
 template <int NT>
@@ -375,7 +377,7 @@ tf32_tap_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_
   __syncthreads();
   const int taps = p.R * p.S;
   const int groups = taps * p.cblocks * p.num_kg;
-  const int num_items = groups * p.splits;
+  const int it0 = p.split0 * groups, it1 = it0 + p.nsplit * groups;
   const int per_split = (p.chunks_total + p.splits - 1) / p.splits;
   // item -> (split, tap, channel block, output group): the items of one split run side by side and re-read its
   // segments from L2
@@ -390,7 +392,7 @@ tf32_tap_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_
       tma_prefetch_desc(&tmap_dy);
       tma_prefetch_desc(&tmap_x);
       int s = 0, ph = 0;
-      for (int it = blockIdx.x; it < num_items; it += gridDim.x) {
+      for (int it = it0 + blockIdx.x; it < it1; it += gridDim.x) {
         TTW_DECODE(it)
         const int dr = tap / p.S - p.ph;
         for (int ch = c_begin; ch < c_end; ++ch) {
@@ -419,8 +421,9 @@ tf32_tap_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_
     const uint32_t off[4] = {xoff0, xoff0 + 8 * TW_XW * 4, xoff0 + 4 * 4, xoff0 + (8 * TW_XW + 4) * 4};
     float acc[NT / 2];
     int s = 0, ph = 0;
-    for (int it = blockIdx.x; it < num_items; it += gridDim.x) {
+    for (int it = it0 + blockIdx.x; it < it1; it += gridDim.x) {
       TTW_DECODE(it)
+      float* dw = p.dw + (size_t)(sp - p.split0) * p.slice_stride;   // the items of one split add disjoint blocks
       const int dx = tap % p.S - p.pw;
       for (int ch = c_begin; ch < c_end; ++ch) {
         mbar_wait(&full[s], ph);
@@ -457,7 +460,7 @@ tf32_tap_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
                 const int k = kg * NT + 8 * j + 2 * t4 + e;
-                if (k < p.K) atomicAdd(&p.dw[((size_t)k * p.C + c) * taps + tap], acc[4 * j + 2 * h + e]);
+                if (k < p.K) atomicAdd(&dw[((size_t)k * p.C + c) * taps + tap], acc[4 * j + 2 * h + e]);
               }
           }
         }
@@ -468,7 +471,7 @@ tf32_tap_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_
 }
 
 template <int NT>
-int launch_tap_wgrad(const CUtensorMap& tdy, const CUtensorMap& tx, TapWgParams p, cudaStream_t st) {
+int launch_tap_wgrad(const CUtensorMap& tdy, const CUtensorMap& tx, TapWgParams p, cudaStream_t st, const WgradSlices* sl) {
   constexpr int STAGE = NT * 128 + TW_XBOX;
   p.stages = (TT_SMEM_LIMIT - TT_SMEM_AUX) / STAGE;
   if (p.stages > 6) p.stages = 6;
@@ -489,11 +492,16 @@ int launch_tap_wgrad(const CUtensorMap& tdy, const CUtensorMap& tx, TapWgParams 
     SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TT_SMEM_LIMIT));
     attr_set = true;
   }
-  const long long items = groups * splits;
-  kern<<<(int)(items < sms ? items : sms), TT_THREADS, p.stages * STAGE + TT_SMEM_AUX, st>>>(tdy, tx, p);
-  count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  return SPC_OK;
+  // smin makes up to chunks_total / TW_MAX_CHAIN splits: the deterministic path may need several passes for them
+  return run_slices(sl, p.splits, (size_t)p.K * p.C * p.R * p.S, p.dw, st, [&](int s0, int ns, float* dst, size_t stride) {
+    TapWgParams q = p;
+    q.split0 = s0; q.nsplit = ns; q.dw = dst; q.slice_stride = stride;
+    const long long items = groups * ns;
+    kern<<<(int)(items < sms ? items : sms), TT_THREADS, p.stages * STAGE + TT_SMEM_AUX, st>>>(tdy, tx, q);
+    count_launch();
+    SPC_CHECK_CUDA(cudaGetLastError());
+    return SPC_OK;
+  });
 }
 }  // namespace
 
@@ -526,7 +534,8 @@ int tf32_tap_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* 
 }
 
 // dw[K][C][R][S] += the interior's share (zero padding), with atomics; api.cu adds the halo strips' share
-int tf32_tap_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st) {
+int tf32_tap_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st,
+                   const WgradSlices* sl) {
   TapWgParams p{};
   p.dw = dw; p.C = d->C; p.K = d->K; p.H = d->H; p.R = d->R; p.S = d->S; p.ph = d->pad_h; p.pw = d->pad_w;
   p.segs_row = (d->W + 31) / 32;
@@ -542,11 +551,11 @@ int tf32_tap_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float*
   rc = make_act_tmap4(&tx, x, d->N, d->C, d->H, d->W, 128, TW_XW, false);
   if (rc) return rc;
   switch (NT) {
-    case 16: return launch_tap_wgrad<16>(tdy, tx, p, st);
-    case 32: return launch_tap_wgrad<32>(tdy, tx, p, st);
-    case 64: return launch_tap_wgrad<64>(tdy, tx, p, st);
-    case 128: return launch_tap_wgrad<128>(tdy, tx, p, st);
-    default: return launch_tap_wgrad<256>(tdy, tx, p, st);
+    case 16: return launch_tap_wgrad<16>(tdy, tx, p, st, sl);
+    case 32: return launch_tap_wgrad<32>(tdy, tx, p, st, sl);
+    case 64: return launch_tap_wgrad<64>(tdy, tx, p, st, sl);
+    case 128: return launch_tap_wgrad<128>(tdy, tx, p, st, sl);
+    default: return launch_tap_wgrad<256>(tdy, tx, p, st, sl);
   }
 }
 

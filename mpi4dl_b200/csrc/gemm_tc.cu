@@ -33,7 +33,7 @@ int run_conv_tap_v2(const __nv_bfloat16* wp, int Mpad, int Cpad, const __nv_bflo
 // wgrad_tap.cu: wgrad of the stride-1 tap convolutions (<= 128 channels on both sides), shifts formed in smem
 bool wgrad_tap_supported(int K, int C, int R, int S, int H, int W, int stride);
 int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, int K, int C, int N, int H, int W, int R, int S,
-                  cudaStream_t st);
+                  cudaStream_t st, const WgradSlices* sl);
 
 // gemm_px.cu: pixel-major 1x1 GEMM (output channels as the wgmma N dimension, NT per tile)
 int run_pw_px(int NT, const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& ty, int M, int Cin, int N, int P,
@@ -555,6 +555,8 @@ struct WgParams {
                     // same number of valid rows and the CTAs that share an x chunk stay in lock-step (L2 hits)
   int pb;           // 64-pixel blocks per stage (1, or 2 = "wide" stages for 1x1 layers with multi-page channel planes)
   int dy5, x5;      // wide stages: operand moves as one 5-d box [8-ch group][px block][8 ch][128 B] (see PwParams::x5)
+  int split0, nsplit;       // this launch runs splits [split0, split0 + nsplit)
+  size_t slice_stride;      // split sp adds into dw + (sp - split0) * slice_stride (common.cuh: WgradSlices)
 };
 
 template <int NBLK, int NA>
@@ -578,7 +580,7 @@ pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_consta
   }
   __syncthreads();
   const int ngroups = p.mgroups * p.n_blocks * p.passes;
-  const int num_items = ngroups * p.splits;
+  const int it0 = p.split0 * ngroups, it1 = it0 + p.nsplit * ngroups;
   const int per_split = (p.chunks_total + p.splits - 1) / p.splits;
 
   // item -> (split, tap pass, channel block, m group), split-major: concurrently running CTAs cover all (m group,
@@ -598,7 +600,7 @@ pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_consta
       tma_prefetch_desc(&tmap_dy);
       tma_prefetch_desc(&tmap_x);
       int s = 0, ph = 0;
-      for (int it = blockIdx.x; it < num_items; it += gridDim.x) {
+      for (int it = it0 + blockIdx.x; it < it1; it += gridDim.x) {
         WG_DECODE(it)
         for (int ch = c_begin; ch < c_end; ++ch) {
           const int n = ch / p.chunks_per_image, p0 = (ch % p.chunks_per_image) * (64 * p.pb);
@@ -650,8 +652,9 @@ pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_consta
     const bool live = 64 * wg < p.mrows;       // rows >= mrows of a block are not dY rows of this block
     float acc[NA][NBLK / 2];
     int s = 0, ph = 0;
-    for (int it = blockIdx.x; it < num_items; it += gridDim.x) {
+    for (int it = it0 + blockIdx.x; it < it1; it += gridDim.x) {
       WG_DECODE(it)
+      float* dw = p.dw + (size_t)(sp - p.split0) * p.slice_stride;   // the items of one split add disjoint blocks
       const int nacc = ntap * MG;              // accumulator a = (tap a / MG, dY block a % MG); a >= nacc: not flushed
       int prev = -1;
       for (int ch = c_begin; ch < c_end; ++ch) {
@@ -716,7 +719,7 @@ pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_consta
 #pragma unroll
                   for (int e = 0; e < 2; ++e) {
                     const int c = nb * NBLK + 8 * q + 2 * (lane & 3) + e;
-                    if (c < p.C) atomicAdd(&p.dw[((size_t)k * p.C + c) * p.taps + tap0 + t], acc[a][4 * q + 2 * h + e]);
+                    if (c < p.C) atomicAdd(&dw[((size_t)k * p.C + c) * p.taps + tap0 + t], acc[a][4 * q + 2 * h + e]);
                   }
                 }
               }
@@ -730,7 +733,8 @@ pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_consta
 }
 
 template <int NBLK, int NA>
-int launch_wg(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMap& tx4, WgParams p, cudaStream_t st) {
+int launch_wg(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMap& tx4, WgParams p, cudaStream_t st,
+              const WgradSlices* sl) {
   const int b_slot = (NBLK * 128 + 1023) & ~1023;
   const int TG = NA / p.MG;                // taps per pass (chosen by launch_wg_na)
   p.TG = TG;
@@ -771,28 +775,33 @@ int launch_wg(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMap& 
     SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
     attr_set = true;
   }
-  const int items = groups * p.splits;
-  kern<<<items < sms ? items : sms, TC_THREADS, smem, st>>>(tdy, tx, tx4, p);
-  count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  return SPC_OK;
+  return run_slices(sl, p.splits, (size_t)p.K * p.C * p.taps, p.dw, st, [&](int s0, int ns, float* dst, size_t stride) {
+    WgParams q = p;
+    q.split0 = s0; q.nsplit = ns; q.dw = dst; q.slice_stride = stride;
+    const int items = groups * ns;
+    kern<<<items < sms ? items : sms, TC_THREADS, smem, st>>>(tdy, tx, tx4, q);
+    count_launch();
+    SPC_CHECK_CUDA(cudaGetLastError());
+    return SPC_OK;
+  });
 }
 
 // accumulators per item: MG dY blocks x TG taps, a power of two <= WG_ACC / NBLK.  TG: all taps when they fit, else the
 // most that fit the accumulator registers and leave room for >= 2 pipeline stages
 template <int NBLK>
-int launch_wg_na(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMap& tx4, const WgParams& p, cudaStream_t st) {
+int launch_wg_na(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMap& tx4, const WgParams& p, cudaStream_t st,
+                 const WgradSlices* sl) {
   constexpr int NACC = WG_ACC / NBLK;
   const int b_slot = (NBLK * 128 + 1023) & ~1023;
   int na = p.MG;
   while (na * 2 <= NACC && na / p.MG < p.taps &&
          p.MG * A_BLK_BYTES + (na * 2 / p.MG) * b_slot <= (SMEM_LIMIT - SMEM_AUX) / 2)
     na *= 2;
-  if (na == 1) return launch_wg<NBLK, 1>(tdy, tx, tx4, p, st);
-  if (na == 2) return launch_wg<NBLK, 2>(tdy, tx, tx4, p, st);
-  if constexpr (NACC >= 4) { if (na == 4) return launch_wg<NBLK, 4>(tdy, tx, tx4, p, st); }
-  if constexpr (NACC >= 8) { if (na == 8) return launch_wg<NBLK, 8>(tdy, tx, tx4, p, st); }
-  if constexpr (NACC >= 16) { if (na == 16) return launch_wg<NBLK, 16>(tdy, tx, tx4, p, st); }
+  if (na == 1) return launch_wg<NBLK, 1>(tdy, tx, tx4, p, st, sl);
+  if (na == 2) return launch_wg<NBLK, 2>(tdy, tx, tx4, p, st, sl);
+  if constexpr (NACC >= 4) { if (na == 4) return launch_wg<NBLK, 4>(tdy, tx, tx4, p, st, sl); }
+  if constexpr (NACC >= 8) { if (na == 8) return launch_wg<NBLK, 8>(tdy, tx, tx4, p, st, sl); }
+  if constexpr (NACC >= 16) { if (na == 16) return launch_wg<NBLK, 16>(tdy, tx, tx4, p, st, sl); }
   set_error("wgmma wgrad: no kernel for %d accumulators of %d channels", na, NBLK);
   return SPC_EUNSUPPORTED;
 }
@@ -800,7 +809,7 @@ int launch_wg_na(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMa
 // x: activations [N][C][Hin][Wo] (taps == 1: Hin == Ho) or their S column-shifted (and, for
 // stride 2, column-subsampled) copies [S][N][C][Hin][Wo].  Ho x Wo = extent of dy.
 int run_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, int K, int C, int N, int Ho, int Wo, int Hin,
-              int R, int S, int ph, int stride, bool copies, cudaStream_t st) {
+              int R, int S, int ph, int stride, bool copies, cudaStream_t st, const WgradSlices* sl) {
   const int P = Ho * Wo;
   WgParams p{};
   p.dw = dw; p.K = K; p.C = C; p.P = P; p.N = N;
@@ -848,10 +857,10 @@ int run_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, int K,
     if (rc) return rc;
     tx4 = tx;
   }
-  if (p.nblk == 16) return launch_wg_na<16>(tdy, tx, tx4, p, st);
-  if (p.nblk == 32) return launch_wg_na<32>(tdy, tx, tx4, p, st);
-  if (p.nblk == 64) return launch_wg_na<64>(tdy, tx, tx4, p, st);
-  return launch_wg_na<128>(tdy, tx, tx4, p, st);
+  if (p.nblk == 16) return launch_wg_na<16>(tdy, tx, tx4, p, st, sl);
+  if (p.nblk == 32) return launch_wg_na<32>(tdy, tx, tx4, p, st, sl);
+  if (p.nblk == 64) return launch_wg_na<64>(tdy, tx, tx4, p, st, sl);
+  return launch_wg_na<128>(tdy, tx, tx4, p, st, sl);
 }
 
 // ---- 3x3 stride-2 dgrad: the four output-parity classes of dX as channel groups of ONE 2x2-tap
@@ -1236,14 +1245,14 @@ int tc_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* d
 }
 
 int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void* ws, size_t ws_bytes,
-                  cudaStream_t st) {
+                  cudaStream_t st, const WgradSlices* sl) {
   // the kernels accumulate into dw with atomics; api.cu has zeroed it unless the caller accumulates
   const __nv_bfloat16* xb = reinterpret_cast<const __nv_bfloat16*>(x);
   const __nv_bfloat16* dyb = reinterpret_cast<const __nv_bfloat16*>(dy);
   if (d->R * d->S > 1) {
     const int cs = d->stride_h;
     if (wgrad_tap_supported(d->K, d->C, d->R, d->S, d->H, d->W, cs))
-      return run_wgrad_tap(xb, dyb, dw, d->K, d->C, d->N, d->H, d->W, d->R, d->S, st);
+      return run_wgrad_tap(xb, dyb, dw, d->K, d->C, d->N, d->H, d->W, d->R, d->S, st, sl);
     const bool copies = d->S > 1 || cs > 1;
     if (copies) {
       SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 2), "wgmma wgrad: workspace too small");
@@ -1252,7 +1261,7 @@ int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* 
       if (rc) return rc;
       xb = reinterpret_cast<const __nv_bfloat16*>(xs);
     }
-    return run_wgrad(xb, dyb, dw, d->K, d->C, d->N, d->H / cs, d->W / cs, d->H, d->R, d->S, d->pad_h, cs, copies, st);
+    return run_wgrad(xb, dyb, dw, d->K, d->C, d->N, d->H / cs, d->W / cs, d->H, d->R, d->S, d->pad_h, cs, copies, st, sl);
   }
   if (is_s2(d)) {
     SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 2), "wgmma wgrad: workspace too small");
@@ -1260,9 +1269,9 @@ int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* 
     int rc = launch_resample(false, x, xs, (size_t)d->N * d->C, d->H, d->W, st);
     if (rc) return rc;
     return run_wgrad(reinterpret_cast<const __nv_bfloat16*>(xs), dyb, dw, d->K, d->C, d->N, 1, (d->H / 2) * (d->W / 2), 1,
-                     1, 1, 0, 1, false, st);
+                     1, 1, 0, 1, false, st, sl);
   }
-  return run_wgrad(xb, dyb, dw, d->K, d->C, d->N, 1, d->H * d->W, 1, 1, 1, 0, 1, false, st);
+  return run_wgrad(xb, dyb, dw, d->K, d->C, d->N, 1, d->H * d->W, 1, 1, 1, 0, 1, false, st, sl);
 }
 
 // Y[M][P] = W[M][Cin] * X[Cin][P] (bf16; w row-major with leading dimension ld) and dW[K][C] += dY[K][P] * X[C][P]^T on
@@ -1275,9 +1284,9 @@ int tc_pw_fwd(const void* w, int ld, int M, int Cin, const void* x, const void* 
                 reinterpret_cast<const __nv_bfloat16*>(bias), reinterpret_cast<__nv_bfloat16*>(y), 1, P, ws, ws_bytes, st,
                 0);
 }
-int tc_pw_wgrad(const void* x, const void* dy, float* dw, int K, int C, int P, cudaStream_t st) {
+int tc_pw_wgrad(const void* x, const void* dy, float* dw, int K, int C, int P, cudaStream_t st, const WgradSlices* sl) {
   return run_wgrad(reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(dy), dw, K, C, 1, 1, P, 1, 1, 1,
-                   0, 1, false, st);
+                   0, 1, false, st, sl);
 }
 
 int make_tmap_ex(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,

@@ -374,6 +374,8 @@ struct Tf32WgParams {
   int splits;         // pixel-range splits per item
   int chunks_total, chunks_per_image;   // 32-pixel chunks
   int stages;
+  int split0, nsplit;       // this launch runs splits [split0, split0 + nsplit)
+  size_t slice_stride;      // split sp adds into dw + (sp - split0) * slice_stride (common.cuh: WgradSlices)
 };
 
 template <int NBLK, int MG>
@@ -396,7 +398,7 @@ tf32_pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_c
   }
   __syncthreads();
   const int ngroups = p.mgroups * p.n_blocks;
-  const int num_items = ngroups * p.splits;
+  const int it0 = p.split0 * ngroups, it1 = it0 + p.nsplit * ngroups;
   const int per_split = (p.chunks_total + p.splits - 1) / p.splits;
   // item -> (split, channel block, m group); concurrently running CTAs cover all groups of the SAME pixel range, so
   // the chunks every group re-reads come from L2
@@ -410,7 +412,7 @@ tf32_pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_c
       tma_prefetch_desc(&tmap_dy);
       tma_prefetch_desc(&tmap_x);
       int s = 0, ph = 0;
-      for (int it = blockIdx.x; it < num_items; it += gridDim.x) {
+      for (int it = it0 + blockIdx.x; it < it1; it += gridDim.x) {
         TWG_DECODE(it)
         for (int ch = c_begin; ch < c_end; ++ch) {
           const int n = ch / p.chunks_per_image, p0 = (ch % p.chunks_per_image) * 32;
@@ -430,8 +432,9 @@ tf32_pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_c
     const bool live = 64 * wg < p.mrows;   // rows >= mrows of a block are not dY rows of this block
     float acc[MG][NBLK / 2];
     int s = 0, ph = 0;
-    for (int it = blockIdx.x; it < num_items; it += gridDim.x) {
+    for (int it = it0 + blockIdx.x; it < it1; it += gridDim.x) {
       TWG_DECODE(it)
+      float* dw = p.dw + (size_t)(sp - p.split0) * p.slice_stride;   // the items of one split add disjoint blocks
       int prev = -1;
       for (int ch = c_begin; ch < c_end; ++ch) {
         mbar_wait(&full[s], ph);
@@ -471,7 +474,7 @@ tf32_pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_c
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                   const int c = nb * NBLK + 8 * q + 2 * (lane & 3) + e;
-                  if (c < p.C) atomicAdd(&p.dw[(size_t)k * p.C + c], acc[i][4 * q + 2 * h + e]);
+                  if (c < p.C) atomicAdd(&dw[(size_t)k * p.C + c], acc[i][4 * q + 2 * h + e]);
                 }
               }
             }
@@ -484,7 +487,7 @@ tf32_pw_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dy, const __grid_c
 }
 
 template <int NBLK, int MG>
-int launch_tf32_wg(const CUtensorMap& tdy, const CUtensorMap& tx, Tf32WgParams p, cudaStream_t st) {
+int launch_tf32_wg(const CUtensorMap& tdy, const CUtensorMap& tx, Tf32WgParams p, cudaStream_t st, const WgradSlices* sl) {
   constexpr int STAGE = MG * T_A_BLK + ((NBLK * 128 + 1023) & ~1023);
   p.stages = (T_SMEM_LIMIT - T_SMEM_AUX) / STAGE;
   if (p.stages > 6) p.stages = 6;
@@ -519,24 +522,30 @@ int launch_tf32_wg(const CUtensorMap& tdy, const CUtensorMap& tx, Tf32WgParams p
     SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM_LIMIT));
     attr_set = true;
   }
-  const int items = groups * p.splits;
-  kern<<<items < sms ? items : sms, T_THREADS, smem, st>>>(tdy, tx, p);
-  count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  return SPC_OK;
+  return run_slices(sl, p.splits, (size_t)p.K * p.C, p.dw, st, [&](int s0, int ns, float* dst, size_t stride) {
+    Tf32WgParams q = p;
+    q.split0 = s0; q.nsplit = ns; q.dw = dst; q.slice_stride = stride;
+    const int items = groups * ns;
+    kern<<<items < sms ? items : sms, T_THREADS, smem, st>>>(tdy, tx, q);
+    count_launch();
+    SPC_CHECK_CUDA(cudaGetLastError());
+    return SPC_OK;
+  });
 }
 
 template <int NBLK>
-int launch_tf32_wg_mg(const CUtensorMap& tdy, const CUtensorMap& tx, const Tf32WgParams& p, int MG, cudaStream_t st) {
-  if (MG == 1) return launch_tf32_wg<NBLK, 1>(tdy, tx, p, st);
-  if constexpr (NBLK <= 128) { if (MG == 2) return launch_tf32_wg<NBLK, 2>(tdy, tx, p, st); }
-  if constexpr (NBLK <= 64) { if (MG == 4) return launch_tf32_wg<NBLK, 4>(tdy, tx, p, st); }
+int launch_tf32_wg_mg(const CUtensorMap& tdy, const CUtensorMap& tx, const Tf32WgParams& p, int MG, cudaStream_t st,
+                      const WgradSlices* sl) {
+  if (MG == 1) return launch_tf32_wg<NBLK, 1>(tdy, tx, p, st, sl);
+  if constexpr (NBLK <= 128) { if (MG == 2) return launch_tf32_wg<NBLK, 2>(tdy, tx, p, st, sl); }
+  if constexpr (NBLK <= 64) { if (MG == 4) return launch_tf32_wg<NBLK, 4>(tdy, tx, p, st, sl); }
   set_error("tf32 wgrad: no kernel for %d blocks of %d channels", MG, NBLK);
   return SPC_EUNSUPPORTED;
 }
 
 // dw[K][C] += dy[N][K][P] * x[N][C][P]^T
-int run_tf32_wgrad(const float* x, const float* dy, float* dw, int K, int C, int N, int P, cudaStream_t st) {
+int run_tf32_wgrad(const float* x, const float* dy, float* dw, int K, int C, int N, int P, cudaStream_t st,
+                   const WgradSlices* sl) {
   Tf32WgParams p{};
   p.dw = dw; p.K = K; p.C = C;
   // accumulator width: C split evenly over blocks of <= 128 channels, rounded up to an instantiated width
@@ -557,9 +566,9 @@ int run_tf32_wgrad(const float* x, const float* dy, float* dw, int K, int C, int
   if (rc) return rc;
   rc = make_act_tmap_f32(&tx, x, P, C, N, nblk);
   if (rc) return rc;
-  if (nblk == 32) return launch_tf32_wg_mg<32>(tdy, tx, p, MG, st);
-  if (nblk == 64) return launch_tf32_wg_mg<64>(tdy, tx, p, MG, st);
-  return launch_tf32_wg_mg<128>(tdy, tx, p, MG, st);
+  if (nblk == 32) return launch_tf32_wg_mg<32>(tdy, tx, p, MG, st, sl);
+  if (nblk == 64) return launch_tf32_wg_mg<64>(tdy, tx, p, MG, st, sl);
+  return launch_tf32_wg_mg<128>(tdy, tx, p, MG, st, sl);
 }
 
 // ---- stride-2 passes (fp32) -------------------------------------------------------------------------------------------
@@ -669,7 +678,7 @@ int tf32_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void*
 }
 
 int tf32_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void* ws, size_t ws_bytes,
-                    cudaStream_t st) {
+                    cudaStream_t st, const WgradSlices* sl) {
   // accumulates with atomics: api.cu has already zeroed dw when !accumulate
   const float* xf = reinterpret_cast<const float*>(x);
   int P = d->H * d->W;
@@ -681,7 +690,7 @@ int tf32_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float
     xf = sub;
     P = (d->H / 2) * (d->W / 2);
   }
-  return run_tf32_wgrad(xf, reinterpret_cast<const float*>(dy), dw, d->K, d->C, d->N, P, st);
+  return run_tf32_wgrad(xf, reinterpret_cast<const float*>(dy), dw, d->K, d->C, d->N, P, st, sl);
 }
 
 }  // namespace spc

@@ -63,7 +63,11 @@ struct WtParams {
   int nbw;                     // 64-pixel blocks per strip row (strip width = 64 * nbw): rows of few channels are
                                // small, and the TMA loads are latency-bound -> wider strips keep more bytes in flight
   int raw_bytes;               // raw Q row bytes: Qc16 * 160
-  int strips, row_splits, rows_per_split, num_items;   // num_items = N * strips * row_splits * npass
+  int strips, row_splits, rows_per_split;
+  // this launch runs slices (image, strip, row range) [split0, split0 + nsplit), all passes of each; slice s adds into
+  // dw + (s - split0) * slice_stride (common.cuh: WgradSlices)
+  int split0, nsplit;
+  size_t slice_stride;
 };
 
 struct Ring {
@@ -141,6 +145,7 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
     fence_barrier_init();
   }
   __syncthreads();
+  const int it0 = p.split0 * p.npass, it1 = it0 + p.nsplit * p.npass;
 
   // item -> (image n, column strip, row range [ha, hb), tap rectangle = pass)
 #define WT_ITEM(it)                                                               \
@@ -165,7 +170,7 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
       tma_prefetch_desc(&tmap_p);
       tma_prefetch_desc(&tmap_q);
       Ring qr, pr, rr;     // Q ring rows / P rows / raw rows issued so far (global counters across items)
-      for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
+      for (int it = it0 + blockIdx.x; it < it1; it += gridDim.x) {
         WT_ITEM(it)
         (void)s0; (void)ns;
         if (rows <= 0) continue;
@@ -204,7 +209,7 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
       const int tid = threadIdx.x - 12 * 32;
       const int q = tid & 7, c0 = tid >> 3;
       Ring qr, rr;
-      for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
+      for (int it = it0 + blockIdx.x; it < it1; it += gridDim.x) {
         WT_ITEM(it)
         (void)w0; (void)n_; (void)q_first;
         if (rows <= 0) continue;
@@ -253,7 +258,7 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
     const bool wg_lead = (threadIdx.x & 127) == 0;
     float acc[NT][QC / 2];
     Ring qr, pr;          // qr.i = ring index of Q row 0 of the current item
-    for (int it = blockIdx.x; it < p.num_items; it += gridDim.x) {
+    for (int it = it0 + blockIdx.x; it < it1; it += gridDim.x) {
       WT_ITEM(it)
       (void)w0; (void)n_; (void)q_first;
       if (rows <= 0) continue;
@@ -302,6 +307,7 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
         for (int i = rows; i < q_rows; ++i) mbar_arrive(&qt_empty[(qr.i + i) % p.rq]);
       }
       qr.i += q_rows;
+      float* dw = p.dw + (size_t)(rest_ - p.split0) * p.slice_stride;   // the passes of one slice add disjoint taps
 #pragma unroll
       for (int a = 0; a < NT; ++a) {
         if (a < ntaps) {
@@ -318,7 +324,7 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
                   const int qc = 8 * q + 2 * (lane & 3) + e;
                   if (qc < p.Qch) {
                     const int k = p.modeB ? qc : pl, c = p.modeB ? pl : qc;
-                    atomicAdd(&p.dw[(((size_t)k * p.C + c) * p.R + r) * p.S + s], acc[a][4 * q + 2 * h + e]);
+                    atomicAdd(&dw[(((size_t)k * p.C + c) * p.R + r) * p.S + s], acc[a][4 * q + 2 * h + e]);
                   }
                 }
               }
@@ -336,7 +342,8 @@ constexpr int WT_SMEM_AUX = 1024 + 1024;
 inline int rup(int a, int b) { return (a + b - 1) / b * b; }
 
 template <int S, int QC>
-int launch_wt(const CUtensorMap& tp, const CUtensorMap& tq, const WtParams& p, int smem, cudaStream_t st) {
+int launch_wt(const CUtensorMap& tp, const CUtensorMap& tq, const WtParams& p, int smem, cudaStream_t st,
+              const WgradSlices* sl) {
   auto kern = wgrad_tap_kernel<S, QC>;
   static bool attr_set = false;
   if (!attr_set) {
@@ -344,10 +351,16 @@ int launch_wt(const CUtensorMap& tp, const CUtensorMap& tq, const WtParams& p, i
     attr_set = true;
   }
   const int sms = tc_sm_count();
-  kern<<<p.num_items < sms ? p.num_items : sms, WT_THREADS, smem, st>>>(tp, tq, p);
-  count_launch();
-  SPC_CHECK_CUDA(cudaGetLastError());
-  return SPC_OK;
+  const int slices = p.N * p.strips * p.row_splits;
+  return run_slices(sl, slices, (size_t)p.K * p.C * p.R * p.S, p.dw, st, [&](int s0, int ns, float* dst, size_t stride) {
+    WtParams q = p;
+    q.split0 = s0; q.nsplit = ns; q.dw = dst; q.slice_stride = stride;
+    const int items = ns * p.npass;
+    kern<<<items < sms ? items : sms, WT_THREADS, smem, st>>>(tp, tq, q);
+    count_launch();
+    SPC_CHECK_CUDA(cudaGetLastError());
+    return SPC_OK;
+  });
 }
 
 // tap rectangles ("passes") of an R x S filter at most maxt taps each; returns the count (0: no plan)
@@ -385,7 +398,7 @@ bool wgrad_tap_supported(int K, int C, int R, int S, int H, int W, int stride) {
 
 // dw += wgrad(x [N][C][H][W], dy [N][K][H][W]) over the zero-padded tile (pad = (R-1)/2, (S-1)/2), bf16 inputs
 int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, int K, int C, int N, int H, int W, int R, int S,
-                  cudaStream_t st) {
+                  cudaStream_t st, const WgradSlices* sl) {
   WtParams p{};
   p.dw = dw; p.K = K; p.C = C; p.R = R; p.S = S; p.H = H; p.W = W; p.N = N;
   p.ph = (R - 1) / 2; p.pw = (S - 1) / 2;
@@ -461,9 +474,8 @@ int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, in
   }
   p.row_splits = best;
   p.rows_per_split = (H + best - 1) / best;
-  p.num_items = base_items * best;
   const int smem = p.psn * prow + p.rq * qrow_bytes + p.rawn * rawrow + WT_SMEM_AUX;
-#define WT_CASE(s, qc) if (S == s && p.Qc16 == qc) return launch_wt<s, qc>(tp, tq, p, smem, st);
+#define WT_CASE(s, qc) if (S == s && p.Qc16 == qc) return launch_wt<s, qc>(tp, tq, p, smem, st, sl);
 #define WT_CASES(s) WT_CASE(s, 16) WT_CASE(s, 32) WT_CASE(s, 48) WT_CASE(s, 64) WT_CASE(s, 80) WT_CASE(s, 96) \
                     WT_CASE(s, 112) WT_CASE(s, 128)
   WT_CASES(3) WT_CASES(5) WT_CASES(7)

@@ -359,9 +359,12 @@ class _ConvSpatialFn(torch.autograd.Function):
             dw32 = torch.empty(weight.shape, dtype=torch.float32, device=x.device)
             db32 = torch.empty(d.K, dtype=torch.float32, device=x.device) if ctx.has_bias else None
             halo = _lib.make_halo(strips)
-            ws, wsp = _workspace(L.spc_conv_workspace_bytes(C.byref(d), 2), x.device)
-            _lib.check(L.spc_conv2d_wgrad(C.byref(d), _ptr(x), C.byref(halo), _ptr(gy), _ptr(dw32), _ptr(db32), 0,
-                                          wsp, 0 if ws is None else ws.numel(), _stream()), "spc_conv2d_wgrad")
+            # torch.use_deterministic_algorithms(True): the wgrad whose dw / db bits depend on its inputs only
+            det = torch.are_deterministic_algorithms_enabled()
+            name = "spc_conv2d_wgrad_deterministic" if det else "spc_conv2d_wgrad"
+            ws, wsp = _workspace(L.spc_conv_workspace_bytes(C.byref(d), 3 if det else 2), x.device)
+            _lib.check(getattr(L, name)(C.byref(d), _ptr(x), C.byref(halo), _ptr(gy), _ptr(dw32), _ptr(db32), 0,
+                                        wsp, 0 if ws is None else ws.numel(), _stream()), name)
             dw = dw32.to(ctx.param_dtype)
             db = db32.to(ctx.param_dtype) if db32 is not None else None
         if exact:
