@@ -38,6 +38,8 @@ def get_parser():
     p.add_argument("--deterministic", action="store_true",
                    help="torch.use_deterministic_algorithms(True): bit-reproducible steps, the convolution weight "
                         "gradients included")
+    p.add_argument("--cuda-graph", action="store_true",
+                   help="run the spatial stages' forward and backward from CUDA graphs captured at the first step")
     p.add_argument("--steps", type=int, default=10)
     return p
 
@@ -91,7 +93,7 @@ def main(kind):
         gens.append(g)
     master = train_spatial_model_master(gens[0], gens[1], batch_size, spatial_size, num_spatial_parts, slice_method, comm1,
                                         comm2, LOCAL_DP_LP=1, parts=parts, ASYNC=True, replications=int(times / 2),
-                                        amp_dtype=amp_dtype, recompute=args.recompute)
+                                        amp_dtype=amp_dtype, recompute=args.recompute, cuda_graph=args.cuda_graph)
     sync = gems_comm.SyncAllreduce(comm1)
     n_img = batch_size * 2 * int(times / 2)
 

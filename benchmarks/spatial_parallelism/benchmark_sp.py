@@ -11,7 +11,8 @@ Same command line as the reference's benchmarks/spatial_parallelism/benchmark_{r
 world size = spatial_size * P + split_size - spatial_size.  Extra flags of this script: --dtype
 {fp32,bf16,bf16-amp} (bf16 puts the spatial convs on the wgmma kernels; bf16-amp too, with fp32
 master weights under torch.autocast), --recompute (recompute the spatial cells in backward from their
-inputs and recorded halo strips), --deterministic (torch.use_deterministic_algorithms(True): bit-reproducible
+inputs and recorded halo strips), --cuda-graph (the spatial stages' forward and backward replayed from
+CUDA graphs), --deterministic (torch.use_deterministic_algorithms(True): bit-reproducible
 steps), --steps N (synthetic batches per epoch, default 10).  APP 3 (synthetic) needs no dataset; APP 1/2 use torchvision like the reference.
 """
 import math
@@ -94,6 +95,8 @@ def get_parser():
     p.add_argument("--deterministic", action="store_true",
                    help="torch.use_deterministic_algorithms(True): bit-reproducible steps, the convolution weight "
                         "gradients included")
+    p.add_argument("--cuda-graph", action="store_true",
+                   help="run the spatial stages' forward and backward from CUDA graphs captured at the first step")
     p.add_argument("--steps", type=int, default=10)
     return p
 
@@ -141,7 +144,8 @@ def main(kind):
     del model
     trainer = train_model_spatial(model_gen, local_rank, batch_size, epochs=1, spatial_size=spatial_size,
                                   num_spatial_parts=num_spatial_parts, parts=parts, ASYNC=True, GEMS_INVERSE=False,
-                                  slice_method=slice_method, mpi_comm=mpi_comm, amp_dtype=amp_dtype, recompute=args.recompute)
+                                  slice_method=slice_method, mpi_comm=mpi_comm, amp_dtype=amp_dtype, recompute=args.recompute,
+                                  cuda_graph=args.cuda_graph)
     sync_allreduce.sync_model_spatial(model_gen)
     is_tile = local_rank < spatial_size * P
     cuda = torch.cuda.is_available()

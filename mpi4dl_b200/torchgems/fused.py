@@ -104,10 +104,17 @@ def bn_relu(x, bn, relu=False):
         mean, var, m = stats[0]
         with torch.no_grad():
             bn.num_batches_tracked += 1
-            mom = bn.momentum if bn.momentum is not None else 1.0 / float(bn.num_batches_tracked)
+            # momentum=None (cumulative average): the factor 1 / num_batches_tracked stays on the device -- reading
+            # the counter on the host would synchronise, which a CUDA-graph capture forbids
+            mom = bn.momentum if bn.momentum is not None else 1.0 / bn.num_batches_tracked.double()
             unbiased = var * (m / max(m - 1.0, 1.0))
-            bn.running_mean.mul_(1 - mom).add_(mean.to(bn.running_mean.dtype), alpha=mom)
-            bn.running_var.mul_(1 - mom).add_(unbiased.to(bn.running_var.dtype), alpha=mom)
+            if bn.momentum is not None:
+                bn.running_mean.mul_(1 - mom).add_(mean.to(bn.running_mean.dtype), alpha=mom)
+                bn.running_var.mul_(1 - mom).add_(unbiased.to(bn.running_var.dtype), alpha=mom)
+            else:
+                keep, mom = (1 - mom).to(bn.running_mean.dtype), mom.to(bn.running_mean.dtype)
+                bn.running_mean.mul_(keep).addcmul_(mean.to(bn.running_mean.dtype), mom)
+                bn.running_var.mul_(keep).addcmul_(unbiased.to(bn.running_var.dtype), mom)
     return z
 
 

@@ -7,14 +7,16 @@ from .mp_pipeline import train_model
 
 class train_model_master:
     def __init__(self, model_gen1, model_gen2, local_rank, batch_size, epochs, criterion=None, optimizer=None, parts=1,
-                 ASYNC=True, replications=1, *, amp_dtype=None, recompute=False):
+                 ASYNC=True, replications=1, *, amp_dtype=None, recompute=False, cuda_graph=False):
         self.mp_size = self.split_size = model_gen1.split_size
         self.second_rank = self.split_size - local_rank - 1
         # as in the reference (:41-62) both replicas get the default criterion / optimizer
         self.train_model1 = train_model(model_gen1, local_rank, batch_size, epochs, parts=parts, ASYNC=True,
-                                        GEMS_INVERSE=False, amp_dtype=amp_dtype, recompute=recompute)
+                                        GEMS_INVERSE=False, amp_dtype=amp_dtype, recompute=recompute,
+                                        cuda_graph=cuda_graph)
         self.train_model2 = train_model(model_gen2, self.second_rank, batch_size, epochs, parts=parts, ASYNC=True,
-                                        GEMS_INVERSE=True, amp_dtype=amp_dtype, recompute=recompute)
+                                        GEMS_INVERSE=True, amp_dtype=amp_dtype, recompute=recompute,
+                                        cuda_graph=cuda_graph)
         self.parts, self.epochs, self.local_rank = parts, epochs, local_rank
         self.ENABLE_ASYNC = ASYNC
         self.batch_size = batch_size

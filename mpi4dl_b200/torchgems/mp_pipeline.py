@@ -6,7 +6,7 @@ trainer builds on.  Mirrors the reference's public surface (src/torchgems/mp_pip
         .models  .shape_list
     train_model(model_gen, local_rank, batch_size, epochs, criterion=None, optimizer=None,
                 parts=1, ASYNC=True, GEMS_INVERSE=False, *, amp_dtype=None,
-                recompute=False)                                                  :171-538
+                recompute=False, cuda_graph=False)                                :171-538
         .run_step(x, y) -> (loss, corrects)  .forward_pass  .backward_pass  .update
 
 Host-side orchestration only (no kernels): activations travel forward and their gradients
@@ -27,6 +27,7 @@ import torch.nn as nn
 import torch.optim as optim
 from torch.nn.parallel import DistributedDataParallel as DDP
 
+from . import graphs
 from .recompute import checkpoint_spatial_cells
 
 
@@ -117,14 +118,20 @@ class model_generator:
 
 class train_model:
     def __init__(self, model_gen, local_rank, batch_size, epochs, criterion=None, optimizer=None, parts=1, ASYNC=True,
-                 GEMS_INVERSE=False, *, amp_dtype=None, recompute=False):
+                 GEMS_INVERSE=False, *, amp_dtype=None, recompute=False, cuda_graph=False):
         """amp_dtype=torch.bfloat16: the forward of this stage runs under torch.autocast with fp32 parameters (fp32
         master weights, gradients and optimizer); activations and their gradients travel in bf16.
         recompute=True: the cells of this stage that contain a spatial layer keep only their inputs and received halo
-        strips for backward and run their forward again there (torchgems.recompute.checkpoint_spatial_cells)."""
+        strips for backward and run their forward again there (torchgems.recompute.checkpoint_spatial_cells).
+        cuda_graph=True: a stage that contains a spatial layer runs its forward and backward from CUDA graphs
+        (torchgems.graphs), captured at the first step; sends, receives, the loss and the optimizer stay eager."""
         self.models = model_gen.models
         if recompute:
             checkpoint_spatial_cells(self.models)
+        if cuda_graph:
+            graphs.check_graphable(self.models)
+        self.cuda_graph = cuda_graph and graphs.has_spatial_layer(self.models)
+        self.graphed = None
         self.shape_list = model_gen.shape_list
         self.input_size = model_gen.input_size
         self.parts = parts
@@ -247,14 +254,23 @@ class train_model:
             return contextlib.nullcontext()
         return torch.autocast(self.device.type, dtype=self.amp_dtype)
 
+    def _run_stage(self, input_x, part_number):
+        """The stage's forward: eager, or replayed from the micro-batch's CUDA graph.  The graphs are captured at the
+        first call, on every tile of the stage at the same step (graph_stage is collective over them)."""
+        if not self.cuda_graph:
+            with self._autocast():
+                return self.models(input_x)
+        if self.graphed is None:
+            self.graphed = graphs.graph_stage(self.models, [input_x] * self.parts, amp_dtype=self.amp_dtype)
+        return self.graphed(input_x, part_number)
+
     def forward_pass(self, data_x, data_y, part_number=0):
         if self.split_rank == 0:
             input_x = data_x
         else:
             self.receive_input_async(part_number)
             input_x = self.input_x_list[part_number]
-        with self._autocast():
-            y = self.models(input_x)
+        y = self._run_stage(input_x, part_number)
         if self.split_rank != self.split_size - 1:
             self.send_input_async(y)
             return y, None

@@ -80,9 +80,7 @@ class _Replay:
         self.rec = rec
 
     def __enter__(self):
-        self.bn = [m for m in self.rec.module.modules() if isinstance(m, _BatchNorm) and m.track_running_stats and
-                   m.running_mean is not None]
-        self.saved = [(m.running_mean.clone(), m.running_var.clone(), m.num_batches_tracked.clone()) for m in self.bn]
+        self.saved = save_batchnorm_buffers(self.rec.module)
         self.rec.replaying, self.rec._pos = True, 0
         self.prev = spatial._set_halo_recorder(self.rec)
 
@@ -90,12 +88,24 @@ class _Replay:
         # also on the early stop of torch.utils.checkpoint, which ends the recompute with an exception
         spatial._set_halo_recorder(self.prev)
         self.rec.replaying = False
-        with torch.no_grad():
-            for m, (mean, var, n) in zip(self.bn, self.saved):
-                m.running_mean.copy_(mean)
-                m.running_var.copy_(var)
-                m.num_batches_tracked.copy_(n)
-        self.bn = self.saved = None
+        restore_batchnorm_buffers(self.saved)
+        self.saved = None
+
+
+def save_batchnorm_buffers(module):
+    """Copies of the running buffers of every BatchNorm in `module` (fused bn_relu or plain nn.BatchNorm2d), for
+    restore_batchnorm_buffers: a forward that must not count as a training step (a recompute, a CUDA-graph warm-up)
+    runs between the two."""
+    return [(m, m.running_mean.clone(), m.running_var.clone(), m.num_batches_tracked.clone()) for m in module.modules()
+            if isinstance(m, _BatchNorm) and m.track_running_stats and m.running_mean is not None]
+
+
+def restore_batchnorm_buffers(saved):
+    with torch.no_grad():
+        for m, mean, var, n in saved:
+            m.running_mean.copy_(mean)
+            m.running_var.copy_(var)
+            m.num_batches_tracked.copy_(n)
 
 
 def _flatten(args):
@@ -130,8 +140,10 @@ def _checkpointed_forward(self, *args):
         return cls_forward(self, *args)
     flat, spec = _flatten(args)
     rec = _HaloRecorder(self)
+    # preserve_rng_state=False: the spatial cells draw no random numbers, so there is no RNG state to give the
+    # recompute back; saving and restoring it is what a CUDA-graph capture of the region (torchgems.graphs) forbids
     return checkpoint(lambda *t: cls_forward(self, *_unflatten(t, spec)), *flat, use_reentrant=False,
-                      context_fn=rec.contexts)
+                      context_fn=rec.contexts, preserve_rng_state=False)
 
 
 def _has_spatial_layer(module):

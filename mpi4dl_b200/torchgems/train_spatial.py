@@ -8,7 +8,8 @@ surface (src/torchgems/train_spatial.py):
     split_input(inputs, image_size, slice_method, local_rank, num_spatial_parts_list)    :241-290
     train_model_spatial(model_gen, local_rank, batch_size, epochs, spatial_size=1,
                         num_spatial_parts=4, ..., slice_method="square", LOCAL_DP_LP=1,
-                        mpi_comm=None, *, amp_dtype=None, recompute=False)             :293-1440
+                        mpi_comm=None, *, amp_dtype=None, recompute=False,
+                        cuda_graph=False)                                              :293-1440
 
 Rank line of one model replica (P tiles per spatial stage, S spatial stages):
 
@@ -100,7 +101,7 @@ def split_input(inputs, image_size, slice_method, local_rank, num_spatial_parts_
 class train_model_spatial(train_model):
     def __init__(self, model_gen, local_rank, batch_size, epochs, spatial_size=1, num_spatial_parts=4, criterion=None,
                  optimizer=None, parts=1, ASYNC=True, GEMS_INVERSE=False, slice_method="square", LOCAL_DP_LP=1,
-                 mpi_comm=None, *, amp_dtype=None, recompute=False):
+                 mpi_comm=None, *, amp_dtype=None, recompute=False, cuda_graph=False):
         if LOCAL_DP_LP != 1:
             raise NotImplementedError("LOCAL_DP_LP > 1 (data parallelism inside the LP tail) is not built yet")
         self.slice_method = slice_method
@@ -130,7 +131,7 @@ class train_model_spatial(train_model):
         self.is_join = self.split_rank == spatial_size
         super().__init__(model_gen, local_rank, batch_size, epochs, criterion=criterion, optimizer=optimizer,
                          parts=parts, ASYNC=ASYNC, GEMS_INVERSE=GEMS_INVERSE, amp_dtype=amp_dtype,
-                         recompute=recompute)
+                         recompute=recompute, cuda_graph=cuda_graph)
         if self.is_join:
             self.initialize_recv_buffers_joint()
 
@@ -226,8 +227,7 @@ class train_model_spatial(train_model):
             self.receive_input_async(part_number)
             input_x = self.input_x_list[part_number]
         with self._no_sync_ctx(part_number):
-            with self._autocast():
-                y = self.models(input_x)
+            y = self._run_stage(input_x, part_number)
             if self.split_rank != self.split_size - 1:
                 self.send_input_async(y)
                 return y, None

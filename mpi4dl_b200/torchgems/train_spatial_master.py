@@ -6,7 +6,7 @@ src/torchgems/train_spatial_master.py:
     verify_spatial_master_config(slice_method, image_size, num_spatial_parts_list, spatial_size, mp_size)  :33-84
     train_spatial_model_master(model_gen1, model_gen2, batch_size, spatial_size, num_spatial_parts,
                                slice_method, mpi_comm_first, mpi_comm_second, LOCAL_DP_LP, ...,
-                               *, amp_dtype=None, recompute=False)                                          :87-501
+                               *, amp_dtype=None, recompute=False, cuda_graph=False)                        :87-501
         .run_step(inputs, labels)                 two (x replications) passes, one per replica
         .run_step_allreduce(inputs, labels, odd)  the --enable-master-comm-opt protocol: instead of an
                                                   allreduce between the replicas, rank r and its mirror
@@ -34,7 +34,7 @@ def verify_spatial_master_config(slice_method, image_size, num_spatial_parts_lis
 class train_spatial_model_master:
     def __init__(self, model_gen1, model_gen2, batch_size, spatial_size, num_spatial_parts, slice_method, mpi_comm_first,
                  mpi_comm_second, LOCAL_DP_LP, criterion=None, optimizer=None, parts=1, ASYNC=True, replications=1, *,
-                 amp_dtype=None, recompute=False):
+                 amp_dtype=None, recompute=False, cuda_graph=False):
         self.mp_size = mpi_comm_first.mp_size
         self.split_size = model_gen1.split_size
         self.local_rank = mpi_comm_first.local_rank
@@ -47,7 +47,7 @@ class train_spatial_model_master:
         self.flat_params_model2, self.flat_grads_model2 = self._flatten(model_gen2.models, self.model2_size)
         common = dict(epochs=1, spatial_size=spatial_size, num_spatial_parts=num_spatial_parts, criterion=criterion,
                       optimizer=optimizer, parts=parts, ASYNC=ASYNC, slice_method=slice_method, LOCAL_DP_LP=LOCAL_DP_LP,
-                      amp_dtype=amp_dtype, recompute=recompute)
+                      amp_dtype=amp_dtype, recompute=recompute, cuda_graph=cuda_graph)
         self.train_model1 = train_model_spatial(model_gen1, mpi_comm_first.local_rank, batch_size, GEMS_INVERSE=False,
                                                 mpi_comm=mpi_comm_first, **common)
         self.train_model2 = train_model_spatial(model_gen2, mpi_comm_second.local_rank, batch_size, GEMS_INVERSE=True,
