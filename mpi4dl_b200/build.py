@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libspconv.so")
 SOURCES = ["api.cu", "conv_direct.cu", "pool.cu", "halo.cu", "gemm_tc.cu", "conv_tap.cu", "wgrad_tap.cu", "bnrelu.cu",
            "halo_grad.cu", "gemm_tf32.cu", "conv_tap_tf32.cu", "conv_tap_s2_tf32.cu",
-           "gemm_px.cu", "wgrad_reduce.cu"]
+           "gemm_px.cu", "wgrad_reduce.cu", "host.cu"]
 NVCC_FLAGS = [
     "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",

@@ -50,7 +50,34 @@ DirectConvParams fwd_params(const spc_conv_desc* d, const void* x, const spc_hal
   return p;
 }
 
-inline size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
+// The kernel family that runs op (0 fprop, 1 dgrad, 2 wgrad) of d; every entry point below switches on it.
+enum class ConvPath { Direct, Bf16, Tf32Pw, Tf32Tap, Tf32TapS2 };
+
+ConvPath conv_path(const spc_conv_desc* d, int op) {
+  if (d->algo == SPC_ALGO_DIRECT) return ConvPath::Direct;
+  // fp32 storage reaches the tensor cores only when the caller opts in to TF32 (gemm_tf32.cu, conv_tap_tf32.cu,
+  // conv_tap_s2_tf32.cu)
+  if (d->dtype == SPC_F32) {
+    if (d->algo != SPC_ALGO_TF32 && d->algo != SPC_ALGO_TF32_ALL && d->algo != SPC_ALGO_TF32_STRIDED)
+      return ConvPath::Direct;
+    if (tf32_supported(d)) return ConvPath::Tf32Pw;
+    if (d->algo != SPC_ALGO_TF32 && tf32_tap_supported(d)) return ConvPath::Tf32Tap;
+    if (d->algo == SPC_ALGO_TF32_STRIDED && tf32_tap_s2_supported(d)) return ConvPath::Tf32TapS2;
+    return ConvPath::Direct;
+  }
+  return tc_supported(d, op) ? ConvPath::Bf16 : ConvPath::Direct;
+}
+
+// conv_path, or SPC_EUNSUPPORTED when the caller asked for the tensor cores (SPC_ALGO_TCGEN05) and op has none
+int checked_path(const spc_conv_desc* d, int op, ConvPath* path) {
+  *path = conv_path(d, op);
+  if (d->algo == SPC_ALGO_TCGEN05 && *path == ConvPath::Direct) {
+    static const char* const name[3] = {"conv_fwd", "conv_dgrad", "conv_wgrad"};
+    set_error("%s: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path", name[op]);
+    return SPC_EUNSUPPORTED;
+  }
+  return SPC_OK;
+}
 
 // ---- halo fix-up of the tensor-core paths: a small GEMM over the boundary outputs only ------------------------------
 // After the interior pass ran the whole tile with zero padding, only the outputs whose window reaches a received
@@ -153,48 +180,24 @@ void spc_conv_out_shape(const spc_conv_desc* d, int* Ho, int* Wo) {
   if (Wo) *Wo = (d->W + 2 * d->pad_w - d->S) / d->stride_w + 1;
 }
 
-int spc_conv_uses_tcgen05(const spc_conv_desc* d, int op) {
-  if (!d || d->algo == SPC_ALGO_DIRECT) return 0;
-  // fp32 storage reaches the tensor cores only when the caller opts in to TF32 (gemm_tf32.cu, conv_tap_tf32.cu)
-  if (d->dtype == SPC_F32) {
-    if (d->algo != SPC_ALGO_TF32 && d->algo != SPC_ALGO_TF32_ALL && d->algo != SPC_ALGO_TF32_STRIDED) return 0;
-    if (tf32_supported(d)) return 1;
-    if (d->algo != SPC_ALGO_TF32 && tf32_tap_supported(d)) return 1;
-    return (d->algo == SPC_ALGO_TF32_STRIDED && tf32_tap_s2_supported(d)) ? 1 : 0;
-  }
-  return tc_supported(d, op) ? 1 : 0;
-}
-
-// fp32 on the tensor cores: the 1x1 GEMM (gemm_tf32.cu) or the tap kernels of stride 1 (conv_tap_tf32.cu) / stride 2
-// (conv_tap_s2_tf32.cu)
-static bool tf32_pointwise(const spc_conv_desc* d) { return d->R == 1 && d->S == 1; }
-static bool tf32_strided(const spc_conv_desc* d) { return d->stride_h == 2; }
+int spc_conv_uses_tcgen05(const spc_conv_desc* d, int op) { return d && conv_path(d, op) != ConvPath::Direct; }
 
 // Slice copies of the deterministic wgrad: the most slices one launch of this shape's wgrad can have, times the
-// gradient's size, capped at SPC_WGRAD_SLICE_BYTES_MAX (larger launches run in passes, with the same bits):
-//   wgmma / TF32 1x1 kernels: splits <= 2 * SMs / groups and dw <= groups * 128 x 256 elements, so <= 2 * SMs * 32768;
-//   bf16 tap kernel: <= 3 waves of items, or one slice per (image, strip) when those alone fill more;
-//   TF32 tap kernels: >= chunks / 512 splits (the longest chain an item may sum), else <= 2 * SMs;
-//   direct kernel: its CTA columns;  bias: <= 64 chunks of K.
+// gradient's size (each kernel family bounds its own), capped at SPC_WGRAD_SLICE_BYTES_MAX (larger launches run in
+// passes, with the same bits); bias: <= 64 chunks of K.
 static size_t wgrad_slice_bytes(const spc_conv_desc* d) {
-  int Ho, Wo;
-  spc_conv_out_shape(d, &Ho, &Wo);
-  const double wn = (double)d->K * d->C * d->R * d->S, sms = tc_sm_count();
-  const double pw = 2.0 * sms * (wn < 32768.0 ? wn : 32768.0);
-  const auto direct = [&](int rH, int rW) { return (double)wgrad_direct_slices(d->N, d->K, d->C, rH, rW) * wn; };
   double need = 64.0 * d->K;
-  const bool tc = spc_conv_uses_tcgen05(d, 2);
-  if (!tc) {
-    need = fmax(need, direct(Ho, Wo));
-  } else if (d->dtype == SPC_BF16) {
-    const double tap = fmax(3.0 * sms, (double)d->N * (d->W / 64)) * wn;
-    need = fmax(need, d->R * d->S > 1 && d->stride_h == 1 && d->W % 64 == 0 ? fmax(tap, pw) : pw);
-  } else if (d->R * d->S == 1) {
-    need = fmax(need, pw);
-  } else {
-    const double chunks = (double)d->N * Ho * ((Wo + 31) / 32);
-    need = fmax(need, fmax(2.0 * sms, ceil(chunks / 512.0)) * wn);
-    need = fmax(need, fmax(direct(Ho, d->pad_w), direct(d->pad_h, Wo)));   // the boundary rectangles' share
+  switch (conv_path(d, 2)) {
+    case ConvPath::Direct: {
+      int Ho, Wo;
+      spc_conv_out_shape(d, &Ho, &Wo);
+      need = fmax(need, direct_wgrad_slice_floats(d, Ho, Wo));
+      break;
+    }
+    case ConvPath::Bf16: need = fmax(need, tc_wgrad_slice_floats(d)); break;
+    case ConvPath::Tf32Pw: need = fmax(need, tf32_wgrad_slice_floats(d)); break;
+    case ConvPath::Tf32Tap:
+    case ConvPath::Tf32TapS2: need = fmax(need, tf32_tap_wgrad_slice_floats(d)); break;
   }
   return (size_t)fmin(need * sizeof(float), (double)SPC_WGRAD_SLICE_BYTES_MAX);
 }
@@ -202,10 +205,14 @@ static size_t wgrad_slice_bytes(const spc_conv_desc* d) {
 size_t spc_conv_workspace_bytes(const spc_conv_desc* d, int op) {
   if (!d) return 0;
   if (op == 3) return validate(d) ? 0 : al256(spc_conv_workspace_bytes(d, 2)) + al256(wgrad_slice_bytes(d));
-  if (!spc_conv_uses_tcgen05(d, op)) return 0;
-  if (d->dtype == SPC_BF16) return tc_workspace_bytes(d, op);
-  if (tf32_pointwise(d)) return tf32_workspace_bytes(d, op);
-  return tf32_strided(d) ? tf32_tap_s2_workspace_bytes(d, op) : tf32_tap_workspace_bytes(d, op);
+  switch (conv_path(d, op)) {
+    case ConvPath::Direct: return 0;
+    case ConvPath::Bf16: return tc_workspace_bytes(d, op);
+    case ConvPath::Tf32Pw: return tf32_workspace_bytes(d, op);
+    case ConvPath::Tf32Tap: return tf32_tap_workspace_bytes(d, op);
+    case ConvPath::Tf32TapS2: return tf32_tap_s2_workspace_bytes(d, op);
+  }
+  return 0;
 }
 
 // Boundary strips: output rows / columns whose window reaches outside the tile, recomputed from
@@ -223,19 +230,15 @@ static int fwd_boundary(const spc_conv_desc* d, DirectConvParams p, const spc_ha
   return SPC_OK;
 }
 
-static int fwd_interior(const spc_conv_desc* d, const void* x, const void* w, const void* bias, void* y, void* workspace,
-                        size_t workspace_bytes, cudaStream_t st) {
-  const bool tc = spc_conv_uses_tcgen05(d, 0);
-  if (d->algo == SPC_ALGO_TCGEN05 && !tc) {
-    set_error("conv_fwd: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
-    return SPC_EUNSUPPORTED;
+static int fwd_interior(const spc_conv_desc* d, ConvPath path, const void* x, const void* w, const void* bias, void* y,
+                        void* ws, size_t ws_bytes, cudaStream_t st) {
+  switch (path) {
+    case ConvPath::Direct: break;
+    case ConvPath::Bf16: return tc_conv_fwd(d, x, w, bias, y, ws, ws_bytes, st);
+    case ConvPath::Tf32Pw: return tf32_conv_fwd(d, x, w, bias, y, ws, ws_bytes, st);
+    case ConvPath::Tf32Tap: return tf32_tap_fwd(d, x, w, bias, y, ws, ws_bytes, st);
+    case ConvPath::Tf32TapS2: return tf32_tap_s2_fwd(d, x, w, bias, y, ws, ws_bytes, st);
   }
-  if (tc && d->dtype == SPC_F32) {
-    if (tf32_pointwise(d)) return tf32_conv_fwd(d, x, w, bias, y, workspace, workspace_bytes, st);
-    return tf32_strided(d) ? tf32_tap_s2_fwd(d, x, w, bias, y, workspace, workspace_bytes, st)
-                           : tf32_tap_fwd(d, x, w, bias, y, workspace, workspace_bytes, st);
-  }
-  if (tc) return tc_conv_fwd(d, x, w, bias, y, workspace, workspace_bytes, st);
   return launch_conv_direct(fwd_params(d, x, nullptr, w, bias, y), d->dtype, st);
 }
 
@@ -246,9 +249,12 @@ int spc_conv2d_fwd(const spc_conv_desc* d, const void* x, const spc_halo* halo, 
   cudaStream_t st = (cudaStream_t)stream;
   if (d->N == 0) return SPC_OK;
   SPC_REQUIRE(x && w && y, "conv_fwd: null tensor pointer");
-  if (!spc_conv_uses_tcgen05(d, 0) && d->algo != SPC_ALGO_TCGEN05)   // direct kernel reads tile + strips in one pass
+  ConvPath path;
+  rc = checked_path(d, 0, &path);
+  if (rc) return rc;
+  if (path == ConvPath::Direct)   // direct kernel reads tile + strips in one pass
     return launch_conv_direct(fwd_params(d, x, halo, w, bias, y), d->dtype, st);
-  rc = fwd_interior(d, x, w, bias, y, workspace, workspace_bytes, st);
+  rc = fwd_interior(d, path, x, w, bias, y, workspace, workspace_bytes, st);
   if (rc) return rc;
   return fwd_boundary(d, fwd_params(d, x, halo, w, bias, y), halo, st);
 }
@@ -259,7 +265,10 @@ int spc_conv2d_fwd_interior(const spc_conv_desc* d, const void* x, const void* w
   if (rc) return rc;
   if (d->N == 0) return SPC_OK;
   SPC_REQUIRE(x && w && y, "conv_fwd_interior: null tensor pointer");
-  return fwd_interior(d, x, w, bias, y, workspace, workspace_bytes, (cudaStream_t)stream);
+  ConvPath path;
+  rc = checked_path(d, 0, &path);
+  if (rc) return rc;
+  return fwd_interior(d, path, x, w, bias, y, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int spc_conv2d_fwd_boundary(const spc_conv_desc* d, const void* x, const spc_halo* halo, const void* w,
@@ -278,17 +287,16 @@ int spc_conv2d_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void
   cudaStream_t st = (cudaStream_t)stream;
   if (d->N == 0) return SPC_OK;
   SPC_REQUIRE(dy && w && dx, "conv_dgrad: null tensor pointer");
-  const bool tc = spc_conv_uses_tcgen05(d, 1);
-  if (d->algo == SPC_ALGO_TCGEN05 && !tc) {
-    set_error("conv_dgrad: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
-    return SPC_EUNSUPPORTED;
+  ConvPath path;
+  rc = checked_path(d, 1, &path);
+  if (rc) return rc;
+  switch (path) {
+    case ConvPath::Direct: break;
+    case ConvPath::Bf16: return tc_conv_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
+    case ConvPath::Tf32Pw: return tf32_conv_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
+    case ConvPath::Tf32Tap: return tf32_tap_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
+    case ConvPath::Tf32TapS2: return tf32_tap_s2_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
   }
-  if (tc && d->dtype == SPC_F32) {
-    if (tf32_pointwise(d)) return tf32_conv_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
-    return tf32_strided(d) ? tf32_tap_s2_dgrad(d, dy, w, dx, workspace, workspace_bytes, st)
-                           : tf32_tap_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
-  }
-  if (tc) return tc_conv_dgrad(d, dy, w, dx, workspace, workspace_bytes, st);
 
   int Ho, Wo;
   spc_conv_out_shape(d, &Ho, &Wo);
@@ -329,6 +337,25 @@ int spc_conv2d_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void
   return SPC_OK;
 }
 
+// The halo pixels' share of dw (exact by linearity) after an interior pass with zero padding: the direct kernel over the
+// outputs whose windows reach a strip, reading the strips through the halo-only view (zero inside the tile)
+static int wgrad_boundary_direct(const spc_conv_desc* d, const spc_halo* halo, const void* dy, float* dw, int Ho, int Wo,
+                                 cudaStream_t st, const WgradSlices* sl) {
+  BoundaryRects b;
+  if (!has_halo(halo) || !boundary_rects(d, halo, Ho, Wo, &b)) return SPC_OK;
+  for (int i = 0; i < b.n; ++i) {
+    DirectWgradParams q{};
+    q.in = make_view(nullptr, halo, d->N, d->C, d->H, d->W, d->pad_h, d->pad_w);
+    q.dy = dy; q.dw = dw;
+    q.K = d->K; q.R = d->R; q.S = d->S; q.sh = d->stride_h; q.sw = d->stride_w; q.ph = d->pad_h; q.pw = d->pad_w;
+    q.Ho = Ho; q.Wo = Wo;
+    q.ry0 = b.y0[i]; q.rx0 = b.x0[i]; q.rH = b.y1[i] - b.y0[i]; q.rW = b.x1[i] - b.x0[i];
+    const int rc = launch_wgrad_direct(q, SPC_F32, st, sl);
+    if (rc) return rc;
+  }
+  return SPC_OK;
+}
+
 // sl == nullptr: every kernel adds straight into dw / db; else through slice copies summed in order (common.cuh)
 static int wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo, const void* dy, float* dw, float* db,
                  int accumulate, void* workspace, size_t workspace_bytes, cudaStream_t st, const WgradSlices* sl) {
@@ -341,50 +368,36 @@ static int wgrad(const spc_conv_desc* d, const void* x, const spc_halo* halo, co
     if (db && !accumulate) SPC_CHECK_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * d->K, st));
     return SPC_OK;
   }
-  const bool tc = spc_conv_uses_tcgen05(d, 2);
-  if (d->algo == SPC_ALGO_TCGEN05 && !tc) {
-    set_error("conv_wgrad: SPC_ALGO_TCGEN05 requested but the shape is not supported by the tensor-core path");
-    return SPC_EUNSUPPORTED;
-  }
-  if (tc && d->dtype == SPC_F32 && tf32_pointwise(d)) {
-    // 1x1: no output window reaches a halo strip, so there is nothing to add for the strips
-    rc = tf32_conv_wgrad(d, x, dy, dw, workspace, workspace_bytes, st, sl);
-    if (rc) return rc;
-  } else if (tc && d->dtype == SPC_F32) {
-    rc = tf32_strided(d) ? tf32_tap_s2_wgrad(d, x, dy, dw, st, sl) : tf32_tap_wgrad(d, x, dy, dw, st, sl);
-    if (rc) return rc;
-    // the halo pixels' share (exact by linearity): the direct kernel over the outputs whose windows reach a strip,
-    // reading the strips through the halo-only view (zero inside the tile)
-    BoundaryRects b;
-    if (has_halo(halo) && boundary_rects(d, halo, Ho, Wo, &b)) {
-      for (int i = 0; i < b.n; ++i) {
-        DirectWgradParams q{};
-        q.in = make_view(nullptr, halo, d->N, d->C, d->H, d->W, d->pad_h, d->pad_w);
-        q.dy = dy; q.dw = dw;
-        q.K = d->K; q.R = d->R; q.S = d->S; q.sh = d->stride_h; q.sw = d->stride_w; q.ph = d->pad_h; q.pw = d->pad_w;
-        q.Ho = Ho; q.Wo = Wo;
-        q.ry0 = b.y0[i]; q.rx0 = b.x0[i]; q.rH = b.y1[i] - b.y0[i]; q.rW = b.x1[i] - b.x0[i];
-        rc = launch_wgrad_direct(q, SPC_F32, st, sl);
-        if (rc) return rc;
-      }
+  ConvPath path;
+  rc = checked_path(d, 2, &path);
+  if (rc) return rc;
+  switch (path) {
+    case ConvPath::Direct: {
+      DirectWgradParams p{};
+      p.in = make_view(x, halo, d->N, d->C, d->H, d->W, d->pad_h, d->pad_w);
+      p.dy = dy; p.dw = dw;
+      p.K = d->K; p.R = d->R; p.S = d->S; p.sh = d->stride_h; p.sw = d->stride_w; p.ph = d->pad_h; p.pw = d->pad_w;
+      p.Ho = Ho; p.Wo = Wo;
+      rc = launch_wgrad_direct(p, d->dtype, st, sl);
+      break;
     }
-  } else if (tc) {
-    rc = tc_conv_wgrad(d, x, dy, dw, workspace, workspace_bytes, st, sl);
-    if (rc) return rc;
-    // add the halo pixels' contribution (exact by linearity): boundary GEMM over the outputs whose windows reach a strip
-    if (has_halo(halo)) {
-      rc = boundary_wgrad_tc(d, halo, dy, dw, st, sl);
-      if (rc) return rc;
-    }
-  } else {
-    DirectWgradParams p{};
-    p.in = make_view(x, halo, d->N, d->C, d->H, d->W, d->pad_h, d->pad_w);
-    p.dy = dy; p.dw = dw;
-    p.K = d->K; p.R = d->R; p.S = d->S; p.sh = d->stride_h; p.sw = d->stride_w; p.ph = d->pad_h; p.pw = d->pad_w;
-    p.Ho = Ho; p.Wo = Wo;
-    rc = launch_wgrad_direct(p, d->dtype, st, sl);
-    if (rc) return rc;
+    case ConvPath::Bf16:
+      rc = tc_conv_wgrad(d, x, dy, dw, workspace, workspace_bytes, st, sl);
+      // add the halo pixels' contribution (exact by linearity): boundary GEMM over the outputs whose windows reach a
+      // strip
+      if (!rc && has_halo(halo)) rc = boundary_wgrad_tc(d, halo, dy, dw, st, sl);
+      break;
+    case ConvPath::Tf32Pw:   // 1x1: no output window reaches a halo strip, so there is nothing to add for the strips
+      rc = tf32_conv_wgrad(d, x, dy, dw, workspace, workspace_bytes, st, sl);
+      break;
+    case ConvPath::Tf32Tap:
+    case ConvPath::Tf32TapS2:
+      rc = path == ConvPath::Tf32Tap ? tf32_tap_wgrad(d, x, dy, dw, workspace, workspace_bytes, st, sl)
+                                     : tf32_tap_s2_wgrad(d, x, dy, dw, workspace, workspace_bytes, st, sl);
+      if (!rc) rc = wgrad_boundary_direct(d, halo, dy, dw, Ho, Wo, st, sl);
+      break;
   }
+  if (rc) return rc;
   if (db) return launch_bias_grad(dy, db, d->N, d->K, Ho * Wo, d->dtype, accumulate, st, sl);
   return SPC_OK;
 }

@@ -114,7 +114,17 @@ inline TileView make_view(const void* x, const spc_halo* halo, int N, int C, int
 }
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
+inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
+inline size_t align1k(size_t b) { return (b + 1023) & ~(size_t)1023; }
+inline size_t al256(size_t b) { return (b + 255) & ~(size_t)255; }
 inline size_t dtype_size(int dt) { return dt == SPC_BF16 ? 2 : 4; }
+inline bool is_s2(const spc_conv_desc* d) { return d->stride_h == 2 && d->stride_w == 2; }
+
+// ---- host.cu ------------------------------------------------------------------------------------------------------
+int sm_count();   // SMs of the current device, cached; 132 (the H100 SXM's) when no device answers
+// Opt kernel in to `bytes` of dynamic shared memory.  Remembered per kernel address: every instantiation of a kernel
+// template is a kernel of its own and needs its own opt-in.
+int allow_dynamic_smem(const void* kernel, int bytes);
 
 // ---- deterministic wgrad (spc_conv2d_wgrad_deterministic): wgrad_reduce.cu ------------------------------------------
 // Every wgrad kernel flushes its partial sums with fp32 atomics.  Its work is cut into slices (a pixel-range split, an
@@ -183,8 +193,9 @@ struct DirectWgradParams {
 int launch_wgrad_direct(const DirectWgradParams& p, int dtype, cudaStream_t st, const WgradSlices* sl = nullptr);
 int launch_bias_grad(const void* dy, float* db, int N, int K, int HW, int dtype, int accumulate, cudaStream_t st,
                      const WgradSlices* sl = nullptr);
-// CTA columns (slices) of launch_wgrad_direct over an output rectangle of rH x rW; 0 if empty
-int wgrad_direct_slices(int N, int K, int C, int rH, int rW);
+// The most slice-copy floats one launch_wgrad_direct of d over an output rectangle of rH x rW can need: its CTA columns
+// times the gradient's size
+double direct_wgrad_slice_floats(const spc_conv_desc* d, int rH, int rW);
 
 // ---- halo fix-up as a small GEMM over the boundary outputs only (halo.cu kernels, api.cu orchestration) ----------
 void* boundary_scratch(size_t bytes);   // grow-only device scratch of the fix-up's operands
@@ -219,7 +230,16 @@ int tc_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* d
                   size_t ws_bytes, cudaStream_t st);
 int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void* ws,
                   size_t ws_bytes, cudaStream_t st, const WgradSlices* sl = nullptr);
-int tc_sm_count();
+// the most slice-copy floats one launch of tc_conv_wgrad can need (an upper bound its planners keep to)
+double tc_wgrad_slice_floats(const spc_conv_desc* d);
+
+// ---- bf16 tap convolutions without shifted copies (stride 1, <= 128 channels): conv_tap.cu, wgrad_tap.cu ----------
+bool tap_v2_supported(int M, int Cin, int R, int S, int H, int W, int N, int stride);
+int run_conv_tap_v2(const __nv_bfloat16* wp, int Mpad, int Cpad, const __nv_bfloat16* x, const __nv_bfloat16* bias,
+                    __nv_bfloat16* y, int M, int Cin, int R, int S, int ph, int H, int W, int N, cudaStream_t st);
+bool wgrad_tap_supported(int K, int C, int R, int S, int H, int W, int stride);
+int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, int K, int C, int N, int H, int W, int R, int S,
+                  cudaStream_t st, const WgradSlices* sl);
 
 // ---- fp32 1x1 convolutions on TF32 wgmma (SPC_ALGO_TF32): gemm_tf32.cu ---------------------------------------------
 bool tf32_supported(const spc_conv_desc* d);
@@ -230,6 +250,8 @@ int tf32_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void*
                     cudaStream_t st);
 int tf32_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void* ws, size_t ws_bytes,
                     cudaStream_t st, const WgradSlices* sl = nullptr);
+// the most slice-copy floats one launch of tf32_conv_wgrad can need
+double tf32_wgrad_slice_floats(const spc_conv_desc* d);
 
 // ---- fp32 stride-1 multi-tap convolutions on TF32 wgmma (SPC_ALGO_TF32_ALL): conv_tap_tf32.cu ----------------------
 bool tf32_tap_supported(const spc_conv_desc* d);
@@ -239,8 +261,11 @@ int tf32_tap_fwd(const spc_conv_desc* d, const void* x, const void* w, const voi
 int tf32_tap_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* dx, void* ws, size_t ws_bytes,
                    cudaStream_t st);
 // the interior's share of dw (zero padding), added with atomics; api.cu adds the halo strips' share
-int tf32_tap_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st,
-                   const WgradSlices* sl = nullptr);
+int tf32_tap_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void* ws, size_t ws_bytes,
+                   cudaStream_t st, const WgradSlices* sl = nullptr);
+// the most slice-copy floats one launch of tf32_tap_wgrad or tf32_tap_s2_wgrad can need, and one of the direct kernel
+// over a boundary rectangle that adds the strips' share
+double tf32_tap_wgrad_slice_floats(const spc_conv_desc* d);
 
 // ---- fp32 stride-2 multi-tap convolutions on TF32 wgmma (SPC_ALGO_TF32_STRIDED): conv_tap_s2_tf32.cu ---------------
 bool tf32_tap_s2_supported(const spc_conv_desc* d);
@@ -250,7 +275,7 @@ int tf32_tap_s2_fwd(const spc_conv_desc* d, const void* x, const void* w, const 
 int tf32_tap_s2_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* dx, void* ws, size_t ws_bytes,
                       cudaStream_t st);
 // the interior's share of dw (zero padding), added with atomics; api.cu adds the halo strips' share
-int tf32_tap_s2_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st,
-                      const WgradSlices* sl = nullptr);
+int tf32_tap_s2_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void* ws, size_t ws_bytes,
+                      cudaStream_t st, const WgradSlices* sl = nullptr);
 
 }  // namespace spc

@@ -267,12 +267,8 @@ int launch_conv_direct(const DirectConvParams& p, int dtype, cudaStream_t st) {
   dim3 grid((unsigned)((size_t)tiles_x * tiles_y * kblocks), p.in.N);
 #define SPC_LAUNCH_DC2(TT, VV, KK)                                                                                  \
   do {                                                                                                               \
-    static bool attr_set = false;                                                                                    \
-    if (!attr_set) {                                                                                                 \
-      SPC_CHECK_CUDA(cudaFuncSetAttribute(conv_direct_kernel<TT, VV, KK>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                          200 * 1024));                                                              \
-      attr_set = true;                                                                                               \
-    }                                                                                                                \
+    const int rc = allow_dynamic_smem((const void*)conv_direct_kernel<TT, VV, KK>, 200 * 1024);                      \
+    if (rc) return rc;                                                                                               \
     conv_direct_kernel<TT, VV, KK><<<grid, DC_THREADS, smem, st>>>(p, CB, tiles_x, kblocks);                         \
   } while (0)
 #define SPC_LAUNCH_DC(TT, VV)                                          \
@@ -301,9 +297,15 @@ static int direct_tiles_per_cta(int N, int K, int C, int rH, int rW) {
   return tiles_per_cta;
 }
 
-int wgrad_direct_slices(int N, int K, int C, int rH, int rW) {
+// CTA columns (slices) of launch_wgrad_direct over an output rectangle of rH x rW; 0 if empty
+static int wgrad_direct_slices(int N, int K, int C, int rH, int rW) {
   if (rH <= 0 || rW <= 0 || N <= 0) return 0;
   return ceil_div(N * ceil_div(rW, WG_TW) * ceil_div(rH, WG_TH), direct_tiles_per_cta(N, K, C, rH, rW));
+}
+
+double direct_wgrad_slice_floats(const spc_conv_desc* d, int rH, int rW) {
+  const double wn = (double)d->K * d->C * d->R * d->S;
+  return (double)wgrad_direct_slices(d->N, d->K, d->C, rH, rW) * wn;
 }
 
 int launch_wgrad_direct(const DirectWgradParams& p_in, int dtype, cudaStream_t st, const WgradSlices* sl) {
@@ -320,6 +322,9 @@ int launch_wgrad_direct(const DirectWgradParams& p_in, int dtype, cudaStream_t s
   const int ctas_x = wgrad_direct_slices(p.in.N, p.K, p.in.C, p.rH, p.rW);
   const int taps = p.R * p.S;
   const size_t wn = (size_t)p.K * p.in.C * taps;
+  const int rc = allow_dynamic_smem(dtype == SPC_BF16 ? (const void*)wgrad_direct_kernel<__nv_bfloat16>
+                                                     : (const void*)wgrad_direct_kernel<float>, 200 * 1024);
+  if (rc) return rc;
   // slice = CTA column: its tiles are summed in registers, its adds cover disjoint (k, c) blocks
   return run_slices(sl, ctas_x, wn, p.dw, st, [&](int s0, int ns, float* dst, size_t stride) {
     DirectWgradParams q = p;
@@ -328,21 +333,9 @@ int launch_wgrad_direct(const DirectWgradParams& p_in, int dtype, cudaStream_t s
     for (int tap0 = 0; tap0 < taps; tap0 += WG_TAPS) {
       const int nt = taps - tap0 < WG_TAPS ? taps - tap0 : WG_TAPS;
       if (dtype == SPC_BF16) {
-        static bool attr_bf16 = false;
-        if (!attr_bf16) {
-          SPC_CHECK_CUDA(cudaFuncSetAttribute(wgrad_direct_kernel<__nv_bfloat16>,
-                                              cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-          attr_bf16 = true;
-        }
         wgrad_direct_kernel<__nv_bfloat16><<<grid, WG_THREADS, smem, st>>>(q, kblocks, cblocks, tiles_x, tiles_y,
                                                                            tiles_per_cta, tap0, nt);
       } else {
-        static bool attr_f32 = false;
-        if (!attr_f32) {
-          SPC_CHECK_CUDA(cudaFuncSetAttribute(wgrad_direct_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              200 * 1024));
-          attr_f32 = true;
-        }
         wgrad_direct_kernel<float><<<grid, WG_THREADS, smem, st>>>(q, kblocks, cblocks, tiles_x, tiles_y,
                                                                   tiles_per_cta, tap0, nt);
       }

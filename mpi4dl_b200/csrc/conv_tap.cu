@@ -25,10 +25,6 @@ namespace spc {
 
 using namespace tc;
 
-int make_tmap_ex(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                 const uint32_t* box, int swizzle128);
-int tc_sm_count();
-
 namespace {
 
 constexpr int TAP_THREADS = 640;
@@ -368,8 +364,6 @@ conv_tap_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constan
 constexpr int TAP_SMEM_LIMIT = 222 * 1024;   // of H100's 227 KB per block
 constexpr int TAP_SMEM_AUX = 1024 /*align*/ + 1024 /*barriers*/;
 
-inline int round_up_i(int a, int b) { return (a + b - 1) / b * b; }
-
 struct TapPlan {
   int NB;
   TapParams p;
@@ -380,12 +374,12 @@ struct TapPlan {
 bool plan_tap(int M, int Cin, int R, int S, int H, int W, int N, TapPlan* out) {
   TapParams p{};
   p.M = M; p.Cin = Cin; p.H = H; p.W = W; p.N = N; p.R = R;
-  p.mrows = round_up_i(M, 8);
-  p.a_blk = round_up_i(p.mrows * 128, 1024);
+  p.mrows = round_up(M, 8);
+  p.a_blk = round_up(p.mrows * 128, 1024);
   p.kchunks = (Cin + 63) / 64;
   const int taps = R * S;
   const bool shift = S > 1;
-  p.cbox = Cin >= 64 ? 64 : round_up_i(Cin, 16);
+  p.cbox = Cin >= 64 ? 64 : round_up(Cin, 16);
   p.raw_blk = p.cbox * (shift ? RAW_SHIFT_ROW : 128);
   const int raw_blk = p.raw_blk;
   const int budget = TAP_SMEM_LIMIT - TAP_SMEM_AUX;
@@ -428,12 +422,9 @@ template <int NB, int S, int KS>
 int launch_tap(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& ty, const TapParams& p, int smem,
                cudaStream_t st) {
   auto kern = conv_tap_kernel<NB, S, KS>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TAP_SMEM_LIMIT));
-    attr_set = true;
-  }
-  const int sms = tc_sm_count();
+  const int rc = allow_dynamic_smem((const void*)kern, TAP_SMEM_LIMIT);
+  if (rc) return rc;
+  const int sms = sm_count();
   const int grid = p.num_tiles < sms ? p.num_tiles : sms;
   kern<<<grid, TAP_THREADS, smem, st>>>(tw, tx, ty, p);
   count_launch();
@@ -465,21 +456,22 @@ int run_conv_tap_v2(const __nv_bfloat16* wp, int Mpad, int Cpad, const __nv_bflo
     const uint64_t dims[2] = {(uint64_t)Cpad, (uint64_t)R * S * Mpad};
     const uint64_t strides[2] = {0, (uint64_t)Cpad * 2};
     const uint32_t box[2] = {64, (uint32_t)p.mrows};
-    int rc = make_tmap_ex(&tw, wp, 2, dims, strides, box, 1);
+    int rc = make_tmap(&tw, wp, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
   {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)Cin, (uint64_t)N};
     const uint64_t strides[4] = {0, (uint64_t)W * 2, (uint64_t)H * W * 2, (uint64_t)H * W * Cin * 2};
     const uint32_t box[4] = {(uint32_t)(S > 1 ? 80 : 64), 1, (uint32_t)p.cbox, 1};
-    int rc = make_tmap_ex(&tx, x, 4, dims, strides, box, S > 1 ? 0 : 1);
+    int rc = make_tmap(&tx, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, dims, strides, box,
+                       S > 1 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
   {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)M, (uint64_t)N};
     const uint64_t strides[4] = {0, (uint64_t)W * 2, (uint64_t)H * W * 2, (uint64_t)H * W * M * 2};
     const uint32_t box[4] = {64, 1, 128, 1};
-    int rc = make_tmap_ex(&ty, y, 4, dims, strides, box, 1);
+    int rc = make_tmap(&ty, y, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
 #define TAP_CASE(s, ks) if (S == s && p.cbox == 16 * ks) return launch_tap<2, s, ks>(tw, tx, ty, p, pl.smem, st);

@@ -318,12 +318,9 @@ int launch_s2_gemm(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorM
   }
   SPC_REQUIRE(p.stages >= 2, "tf32 stride-2 tap conv: shared memory budget too small (NT=%d)", NT);
   auto kern = tf32_s2_gemm_kernel<NT, MODE>;
-  static bool attr_set = false;   // per instantiation
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TT_SMEM_LIMIT));
-    attr_set = true;
-  }
-  const int sms = tc_sm_count();
+  const int rc = allow_dynamic_smem((const void*)kern, TT_SMEM_LIMIT);
+  if (rc) return rc;
+  const int sms = sm_count();
   kern<<<p.num_tiles < sms ? p.num_tiles : sms, TT_THREADS, smem, st>>>(tw, tx, ty, p);
   count_launch();
   SPC_CHECK_CUDA(cudaGetLastError());
@@ -393,7 +390,7 @@ int run_s2_gemm(const spc_conv_desc* d, int dgrad, const float* w, const float* 
     const uint64_t dims[2] = {(uint64_t)Cpad, (uint64_t)rblocks * Mpad};
     const uint64_t strides[2] = {0, (uint64_t)Cpad * 4};
     const uint32_t box[2] = {TT_BK, (uint32_t)NT};
-    int rc = make_tmap_f32(&tw, wp, 2, dims, strides, box, true);
+    int rc = make_tmap(&tw, wp, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
   int rc = dgrad ? make_act_tmap4(&tx, x, d->N, Cin, Ho, Wo, TT_BK, S2_DXW, false)
@@ -547,7 +544,7 @@ int launch_s2_wgrad(const CUtensorMap& tdy, const CUtensorMap& tx, S2WgParams p,
   p.stages = (TT_SMEM_LIMIT - TT_SMEM_AUX) / STAGE;
   if (p.stages > 6) p.stages = 6;
   SPC_REQUIRE(p.stages >= 2, "tf32 stride-2 tap wgrad: smem budget");
-  const int sms = tc_sm_count();
+  const int sms = sm_count();
   const long long groups = (long long)p.R * p.S * p.cblocks * p.num_kg;
   // at least two items per SM, at least 8 segments per item, at most TW_MAX_CHAIN segments per item
   long long splits = (2 * sms + groups - 1) / groups;
@@ -558,11 +555,8 @@ int launch_s2_wgrad(const CUtensorMap& tdy, const CUtensorMap& tx, S2WgParams p,
   SPC_REQUIRE(groups * splits < (1ll << 31), "tf32 stride-2 tap wgrad: too many work items");
   p.splits = (int)splits;
   auto kern = tf32_s2_wgrad_kernel<NT>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TT_SMEM_LIMIT));
-    attr_set = true;
-  }
+  const int rc = allow_dynamic_smem((const void*)kern, TT_SMEM_LIMIT);
+  if (rc) return rc;
   // smin makes up to chunks_total / TW_MAX_CHAIN splits: the deterministic path may need several passes for them
   return run_slices(sl, p.splits, (size_t)p.K * p.C * p.R * p.S, p.dw, st, [&](int s0, int ns, float* dst, size_t stride) {
     S2WgParams q = p;
@@ -604,9 +598,10 @@ int tf32_tap_s2_dgrad(const spc_conv_desc* d, const void* dy, const void* w, voi
                      reinterpret_cast<float*>(dx), ws, st);
 }
 
-// dw[K][C][R][S] += the interior's share (zero padding), with atomics; api.cu adds the halo strips' share
-int tf32_tap_s2_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st,
-                   const WgradSlices* sl) {
+// dw[K][C][R][S] += the interior's share (zero padding), with atomics; api.cu adds the halo strips' share.  Needs no
+// workspace.
+int tf32_tap_s2_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void*, size_t, cudaStream_t st,
+                      const WgradSlices* sl) {
   S2WgParams p{};
   const int Ho = d->H / 2, Wo = d->W / 2;
   p.dw = dw; p.C = d->C; p.K = d->K; p.Ho = Ho; p.R = d->R; p.S = d->S; p.ph = d->pad_h; p.pw = d->pad_w;

@@ -270,12 +270,9 @@ int launch_tap_gemm(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensor
   }
   SPC_REQUIRE(p.stages >= 2, "tf32 tap conv: shared memory budget too small (NT=%d steps=%d)", NT, p.steps);
   auto kern = tf32_tap_gemm_kernel<NT, SMALL>;
-  static bool attr_set = false;   // per instantiation
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TT_SMEM_LIMIT));
-    attr_set = true;
-  }
-  const int sms = tc_sm_count();
+  const int rc = allow_dynamic_smem((const void*)kern, TT_SMEM_LIMIT);
+  if (rc) return rc;
+  const int sms = sm_count();
   kern<<<p.num_tiles < sms ? p.num_tiles : sms, TT_THREADS, smem, st>>>(tw, tx, ty, p);
   count_launch();
   SPC_CHECK_CUDA(cudaGetLastError());
@@ -308,7 +305,7 @@ int run_tap_gemm(const spc_conv_desc* d, int dgrad, const float* w, const float*
     const uint64_t dims[2] = {(uint64_t)Cpad, (uint64_t)rblocks * Mpad};
     const uint64_t strides[2] = {0, (uint64_t)Cpad * 4};
     const uint32_t box[2] = {TT_BK, (uint32_t)NT};
-    int rc = make_tmap_f32(&tw, wp, 2, dims, strides, box, true);
+    int rc = make_tmap(&tw, wp, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
   int rc = make_act_tmap4(&tx, x, d->N, Cin, d->H, d->W, small ? 8 : TT_BK, TT_XW, false);
@@ -476,7 +473,7 @@ int launch_tap_wgrad(const CUtensorMap& tdy, const CUtensorMap& tx, TapWgParams 
   p.stages = (TT_SMEM_LIMIT - TT_SMEM_AUX) / STAGE;
   if (p.stages > 6) p.stages = 6;
   SPC_REQUIRE(p.stages >= 2, "tf32 tap wgrad: smem budget");
-  const int sms = tc_sm_count();
+  const int sms = sm_count();
   const long long groups = (long long)p.R * p.S * p.cblocks * p.num_kg;
   // at least two items per SM, at least 8 segments per item, at most TW_MAX_CHAIN segments per item
   long long splits = (2 * sms + groups - 1) / groups;
@@ -487,11 +484,8 @@ int launch_tap_wgrad(const CUtensorMap& tdy, const CUtensorMap& tx, TapWgParams 
   SPC_REQUIRE(groups * splits < (1ll << 31), "tf32 tap wgrad: too many work items");
   p.splits = (int)splits;
   auto kern = tf32_tap_wgrad_kernel<NT>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TT_SMEM_LIMIT));
-    attr_set = true;
-  }
+  const int rc = allow_dynamic_smem((const void*)kern, TT_SMEM_LIMIT);
+  if (rc) return rc;
   // smin makes up to chunks_total / TW_MAX_CHAIN splits: the deterministic path may need several passes for them
   return run_slices(sl, p.splits, (size_t)p.K * p.C * p.R * p.S, p.dw, st, [&](int s0, int ns, float* dst, size_t stride) {
     TapWgParams q = p;
@@ -533,8 +527,9 @@ int tf32_tap_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* 
                       reinterpret_cast<float*>(dx), ws, st);
 }
 
-// dw[K][C][R][S] += the interior's share (zero padding), with atomics; api.cu adds the halo strips' share
-int tf32_tap_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, cudaStream_t st,
+// dw[K][C][R][S] += the interior's share (zero padding), with atomics; api.cu adds the halo strips' share.  Needs no
+// workspace.
+int tf32_tap_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void*, size_t, cudaStream_t st,
                    const WgradSlices* sl) {
   TapWgParams p{};
   p.dw = dw; p.C = d->C; p.K = d->K; p.H = d->H; p.R = d->R; p.S = d->S; p.ph = d->pad_h; p.pw = d->pad_w;
@@ -557,6 +552,17 @@ int tf32_tap_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float*
     case 128: return launch_tap_wgrad<128>(tdy, tx, p, st, sl);
     default: return launch_tap_wgrad<256>(tdy, tx, p, st, sl);
   }
+}
+
+// Slice copies of the tap wgrads: launch_tap_wgrad and conv_tap_s2_tf32.cu's launch_s2_wgrad make >= chunks /
+// TW_MAX_CHAIN splits (the longest chain an item may sum), else <= 2 * SMs; the direct kernel's launches over the
+// boundary rectangles (api.cu) make their CTA columns
+double tf32_tap_wgrad_slice_floats(const spc_conv_desc* d) {
+  int Ho, Wo;
+  spc_conv_out_shape(d, &Ho, &Wo);
+  const double wn = (double)d->K * d->C * d->R * d->S, chunks = (double)d->N * Ho * ((Wo + 31) / 32);
+  const double interior = fmax(2.0 * sm_count(), ceil(chunks / TW_MAX_CHAIN)) * wn;
+  return fmax(interior, fmax(direct_wgrad_slice_floats(d, Ho, d->pad_w), direct_wgrad_slice_floats(d, d->pad_h, Wo)));
 }
 
 }  // namespace spc

@@ -242,11 +242,8 @@ int launch_px(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& t
   }
   SPC_REQUIRE(p.stages >= 2, "wgmma px conv: shared memory budget too small (NT=%d kchunks=%d)", NT, kchunks);
   auto kern = pw_px_gemm_kernel<NT>;
-  static bool attr_set = false;   // per instantiation
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PX_SMEM_LIMIT));
-    attr_set = true;
-  }
+  const int rc = allow_dynamic_smem((const void*)kern, PX_SMEM_LIMIT);
+  if (rc) return rc;
   kern<<<p.num_tiles < sms ? p.num_tiles : sms, PX_THREADS, smem, st>>>(tw, tx, ty, p);
   count_launch();
   SPC_CHECK_CUDA(cudaGetLastError());

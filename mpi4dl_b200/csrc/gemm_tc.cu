@@ -25,86 +25,12 @@ namespace spc {
 
 using namespace tc;
 
-// conv_tap.cu: tap convolutions (stride 1, <= 128 output channels) without shifted copies
-bool tap_v2_supported(int M, int Cin, int R, int S, int H, int W, int N, int stride);
-int run_conv_tap_v2(const __nv_bfloat16* wp, int Mpad, int Cpad, const __nv_bfloat16* x, const __nv_bfloat16* bias,
-                    __nv_bfloat16* y, int M, int Cin, int R, int S, int ph, int H, int W, int N, cudaStream_t st);
-
-// wgrad_tap.cu: wgrad of the stride-1 tap convolutions (<= 128 channels on both sides), shifts formed in smem
-bool wgrad_tap_supported(int K, int C, int R, int S, int H, int W, int stride);
-int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, int K, int C, int N, int H, int W, int R, int S,
-                  cudaStream_t st, const WgradSlices* sl);
-
-// gemm_px.cu: pixel-major 1x1 GEMM (output channels as the wgmma N dimension, NT per tile)
-int run_pw_px(int NT, const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& ty, int M, int Cin, int N, int P,
-              int x5, int y5, const __nv_bfloat16* bias, int sms, cudaStream_t st);
-
 namespace {
 
 constexpr int TC_THREADS = 384;
 constexpr int BK = 64;                 // channels per pipeline stage (one 128-byte swizzle row of A)
 constexpr int A_BLK_BYTES = 128 * BK * 2;   // one 128-row M block of A per stage: 16 KB
 constexpr int B_BLK_BYTES = BK * 64 * 2;    // one 64-pixel block of B per stage: 8 KB
-
-// ---- host: TMA descriptor encode (driver entry point fetched through the runtime) -------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  }
-  return fn;
-}
-
-// bf16 tensor map, rank <= 4; dims/strides innermost first (strides in BYTES for dims 1..).
-int make_tmap_sw(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                 const uint32_t* box, CUtensorMapSwizzle swz) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled entry point not available");
-    return SPC_ECUDA;
-  }
-  // bind the primary context to this (possibly autograd worker) thread -- once per thread: cudaFree is not
-  // allowed while a stream is being captured into a CUDA graph, and it is not free either
-  static thread_local bool ctx_bound = false;
-  if (!ctx_bound) {
-    if (cudaFree(nullptr) != cudaSuccess) {
-      set_error("wgmma conv: no CUDA context on this thread");
-      return SPC_ECUDA;
-    }
-    ctx_bound = true;
-  }
-  cuuint64_t gd[5], gs[5];
-  cuuint32_t bx[5], es[5];
-  for (int i = 0; i < rank; ++i) {
-    gd[i] = dims[i];
-    bx[i] = box[i];
-    es[i] = 1;
-    if (i > 0) gs[i - 1] = strides_bytes[i];
-  }
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed (%d) rank=%d dims=[%llu,%llu,%llu] strides=[%llu,%llu]", (int)r, rank,
-              (unsigned long long)dims[0], (unsigned long long)(rank > 1 ? dims[1] : 0),
-              (unsigned long long)(rank > 2 ? dims[2] : 0), (unsigned long long)(rank > 1 ? strides_bytes[1] : 0),
-              (unsigned long long)(rank > 2 ? strides_bytes[2] : 0));
-    return SPC_ECUDA;
-  }
-  return SPC_OK;
-}
-
-int make_tmap(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-              const uint32_t* box) {
-  return make_tmap_sw(m, base, rank, dims, strides_bytes, box, CU_TENSOR_MAP_SWIZZLE_128B);
-}
 
 // ---- weight repack: Wp[tap][m][c] (bf16, zero padded to [taps][Mpad][Cpad]) -----------------------
 // element = w[m*sm + c*sc + (flip ? taps-1-tap : tap)]
@@ -335,17 +261,6 @@ pw_gemm_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
   }
 }
 
-inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
-inline int sm_count() {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-  }
-  return sms;
-}
-
 constexpr int SMEM_LIMIT = 222 * 1024;   // of H100's 227 KB per block: room for a small co-resident kernel (halo post/collect)
 constexpr int SMEM_AUX = 1024 /*align*/ + 512 /*barriers*/;
 
@@ -368,11 +283,8 @@ int launch_pw(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& t
   SPC_REQUIRE(p.stages >= 2, "wgmma conv: shared memory budget too small (MB=%d kchunks=%d)", MB, kchunks);
   const int smem = (p.wres ? wres_bytes : 0) + p.stages * stage_bytes + p.out_bufs * OUT_BUF_BYTES + SMEM_AUX;
   auto kern = pw_gemm_kernel<MB>;
-  static bool attr_set = false;   // per instantiation
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
-    attr_set = true;
-  }
+  const int rc = allow_dynamic_smem((const void*)kern, SMEM_LIMIT);
+  if (rc) return rc;
   kern<<<grid, TC_THREADS, smem, st>>>(tw, tx, tx4, ty, p);
   count_launch();
   SPC_CHECK_CUDA(cudaGetLastError());
@@ -383,7 +295,7 @@ int make_act_tmap(CUtensorMap* m, const void* base, int P, int Cc, int N, int bo
   const uint64_t dims[3] = {(uint64_t)P, (uint64_t)Cc, (uint64_t)N};
   const uint64_t strides[3] = {0, (uint64_t)P * 2, (uint64_t)P * Cc * 2};
   const uint32_t box[3] = {64, (uint32_t)box_rows, 1};
-  return make_tmap(m, base, 3, dims, strides, box);
+  return make_tmap(m, base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 // [N][Cc][P] bf16 as (64 px, 8 channels, P/64 pixel blocks, Cc/8 channel groups, N): one box = `groups` channel
@@ -392,7 +304,7 @@ int make_act_tmap5(CUtensorMap* m, const void* base, int P, int Cc, int N, int g
   const uint64_t dims[5] = {64, 8, (uint64_t)P / 64, (uint64_t)Cc / 8, (uint64_t)N};
   const uint64_t strides[5] = {0, (uint64_t)P * 2, 128, (uint64_t)P * 16, (uint64_t)P * Cc * 2};
   const uint32_t box[5] = {64, 8, (uint32_t)blocks, (uint32_t)groups, 1};
-  return make_tmap(m, base, 5, dims, strides, box);
+  return make_tmap(m, base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 int launch_shift_copies(const void* x, void* xs, size_t planes, int H, int W, int S, int pw, int cs, cudaStream_t st);
@@ -473,7 +385,7 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
     const uint64_t dims[2] = {(uint64_t)Cpad, (uint64_t)taps * Mpad};
     const uint64_t strides[2] = {0, (uint64_t)Cpad * 2};
     const uint32_t box[2] = {BK, px ? (uint32_t)nt : 128u};
-    int rc = make_tmap(&tw, wp, 2, dims, strides, box);
+    int rc = make_tmap(&tw, wp, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
   int rc;
@@ -489,7 +401,7 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
     const uint64_t dims[4] = {(uint64_t)Wo, (uint64_t)c.H, (uint64_t)c.Cin, (uint64_t)c.N * (copies ? c.S : 1)};
     const uint64_t strides[4] = {0, (uint64_t)Wo * 2, (uint64_t)c.H * Wo * 2, (uint64_t)c.H * Wo * c.Cin * 2};
     const uint32_t box[4] = {64, 1, BK, 1};
-    rc = make_tmap(&tx4, xsrc, 4, dims, strides, box);
+    rc = make_tmap(&tx4, xsrc, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     tx = tx4;
   } else {
@@ -770,11 +682,8 @@ int launch_wg(const CUtensorMap& tdy, const CUtensorMap& tx, const CUtensorMap& 
   p.splits = splits;
   const int smem = p.stages * stage_bytes + SMEM_AUX;
   auto kern = pw_wgrad_kernel<NBLK, NA>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
-    attr_set = true;
-  }
+  const int rc = allow_dynamic_smem((const void*)kern, SMEM_LIMIT);
+  if (rc) return rc;
   return run_slices(sl, p.splits, (size_t)p.K * p.C * p.taps, p.dw, st, [&](int s0, int ns, float* dst, size_t stride) {
     WgParams q = p;
     q.split0 = s0; q.nsplit = ns; q.dw = dst; q.slice_stride = stride;
@@ -849,7 +758,7 @@ int run_wgrad(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, int K,
     const uint64_t dims[4] = {(uint64_t)Wo, (uint64_t)Hin, (uint64_t)C, (uint64_t)N * (copies ? S : 1)};
     const uint64_t strides[4] = {0, (uint64_t)Wo * 2, (uint64_t)Hin * Wo * 2, (uint64_t)Hin * Wo * C * 2};
     const uint32_t box[4] = {64, 1, (uint32_t)p.nblk, 1};
-    rc = make_tmap(&tx4, x, 4, dims, strides, box);
+    rc = make_tmap(&tx4, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     tx = tx4;
   } else {
@@ -1091,9 +1000,6 @@ int launch_shift_copies(const void* x, void* xs, size_t planes, int H, int W, in
   return SPC_OK;
 }
 
-inline bool is_s2(const spc_conv_desc* d) { return d->stride_h == 2 && d->stride_w == 2; }
-inline size_t align1k(size_t b) { return (b + 1023) & ~(size_t)1023; }
-
 bool tap_shape_ok(const spc_conv_desc* d) {   // odd RxS "same" convs, stride 1 or 2, on 64-pixel output row segments
   if (d->dtype != SPC_BF16) return false;
   if (d->R * d->S == 1 || d->R * d->S > 49) return false;
@@ -1274,6 +1180,16 @@ int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* 
   return run_wgrad(xb, dyb, dw, d->K, d->C, d->N, 1, d->H * d->W, 1, 1, 1, 0, 1, false, st, sl);
 }
 
+// Slice copies of tc_conv_wgrad: pw_wgrad_kernel (launch_wg) makes <= 2 * SMs / groups splits of a gradient of <= groups
+// * 128 x 256 floats, so <= 2 * SMs * 32768 floats; wgrad_tap_kernel (run_wgrad_tap) fills <= 3 waves of items, or
+// makes one slice per (image, strip) when those alone fill more
+double tc_wgrad_slice_floats(const spc_conv_desc* d) {
+  const double wn = (double)d->K * d->C * d->R * d->S, sms = sm_count();
+  const double pw = 2.0 * sms * (wn < 32768.0 ? wn : 32768.0);
+  const double tap = fmax(3.0 * sms, (double)d->N * (d->W / 64)) * wn;
+  return d->R * d->S > 1 && d->stride_h == 1 && d->W % 64 == 0 ? fmax(tap, pw) : pw;
+}
+
 // Y[M][P] = W[M][Cin] * X[Cin][P] (bf16; w row-major with leading dimension ld) and dW[K][C] += dY[K][P] * X[C][P]^T on
 // the pointwise wgmma kernels -- used by the halo fix-up (api.cu), where "channels" are (c, r, s) triples of the
 // filter and "pixels" are the boundary outputs
@@ -1288,12 +1204,5 @@ int tc_pw_wgrad(const void* x, const void* dy, float* dw, int K, int C, int P, c
   return run_wgrad(reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(dy), dw, K, C, 1, 1, P, 1, 1, 1,
                    0, 1, false, st, sl);
 }
-
-int make_tmap_ex(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                 const uint32_t* box, int swizzle128) {
-  return make_tmap_sw(m, base, rank, dims, strides_bytes, box,
-                      swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE);
-}
-int tc_sm_count() { return sm_count(); }
 
 }  // namespace spc

@@ -20,57 +20,6 @@
 
 namespace spc {
 
-int tc_sm_count();
-
-// ---- host: fp32 TMA descriptors ----------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-// fp32 tensor map with SWIZZLE_128B (swizzle = false: none), rank 2 to 4 (conv_tap_tf32.cu uses it too); dims
-// innermost first, strides in bytes (dims 1..)
-int make_tmap_f32(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                  const uint32_t* box, bool swizzle) {
-  static EncodeTiledFn enc = nullptr;
-  if (!enc) {
-    void* fp = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fp, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      enc = reinterpret_cast<EncodeTiledFn>(fp);
-  }
-  if (!enc) {
-    set_error("cuTensorMapEncodeTiled entry point not available");
-    return SPC_ECUDA;
-  }
-  static thread_local bool ctx_bound = false;   // bind the primary context to this (possibly autograd worker) thread
-  if (!ctx_bound) {
-    if (cudaFree(nullptr) != cudaSuccess) {
-      set_error("tf32 conv: no CUDA context on this thread");
-      return SPC_ECUDA;
-    }
-    ctx_bound = true;
-  }
-  cuuint64_t gd[4], gs[3];
-  cuuint32_t bx[4], es[4];
-  for (int i = 0; i < rank; ++i) {
-    gd[i] = dims[i];
-    bx[i] = box[i];
-    es[i] = 1;
-    if (i > 0) gs[i - 1] = strides_bytes[i];
-  }
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled (fp32) failed (%d) rank=%d dims=[%llu,%llu,%llu]", (int)r, rank,
-              (unsigned long long)dims[0], (unsigned long long)dims[1], (unsigned long long)(rank > 2 ? dims[2] : 0));
-    return SPC_ECUDA;
-  }
-  return SPC_OK;
-}
-
 namespace {
 
 using namespace tc;
@@ -92,16 +41,7 @@ int make_act_tmap_f32(CUtensorMap* m, const void* base, int P, int rows, int N, 
   const uint64_t dims[3] = {(uint64_t)P, (uint64_t)rows, (uint64_t)N};
   const uint64_t strides[3] = {0, (uint64_t)P * 4, (uint64_t)P * rows * 4};
   const uint32_t box[3] = {32, (uint32_t)box_rows, 1};
-  return make_tmap_f32(m, base, 3, dims, strides, box, true);
-}
-
-inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
-inline size_t align1k(size_t b) { return (b + 1023) & ~(size_t)1023; }
-
-__device__ __forceinline__ uint32_t to_tf32(float v) {   // round to nearest, ties away (the low 13 bits become 0)
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-  return r;
+  return make_tmap(m, base, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 // ---- weight repack: Wp[m][c'] = tf32(w[m*sm + c*sc]), zero padded to [Mpad][Cpad] --------------------------------
@@ -306,12 +246,9 @@ int launch_tf32_pw(const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorM
   }
   SPC_REQUIRE(p.stages >= 2, "tf32 conv: shared memory budget too small (NT=%d kchunks=%d)", NT, kchunks);
   auto kern = tf32_pw_gemm_kernel<NT>;
-  static bool attr_set = false;   // per instantiation
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM_LIMIT));
-    attr_set = true;
-  }
-  const int sms = tc_sm_count();
+  const int rc = allow_dynamic_smem((const void*)kern, T_SMEM_LIMIT);
+  if (rc) return rc;
+  const int sms = sm_count();
   kern<<<p.num_tiles < sms ? p.num_tiles : sms, T_THREADS, smem, st>>>(tw, tx, ty, p);
   count_launch();
   SPC_CHECK_CUDA(cudaGetLastError());
@@ -341,7 +278,7 @@ int run_tf32_pw(const float* w, int transpose, int M, int Cin, const float* x, c
     const uint64_t dims[2] = {(uint64_t)Cpad, (uint64_t)Mpad};
     const uint64_t strides[2] = {0, (uint64_t)Cpad * 4};
     const uint32_t box[2] = {T_BK, (uint32_t)NT};
-    int rc = make_tmap_f32(&tw, wp, 2, dims, strides, box, true);
+    int rc = make_tmap(&tw, wp, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
   int rc = make_act_tmap_f32(&tx, x, P, Cin, N, T_BK);
@@ -492,7 +429,7 @@ int launch_tf32_wg(const CUtensorMap& tdy, const CUtensorMap& tx, Tf32WgParams p
   p.stages = (T_SMEM_LIMIT - T_SMEM_AUX) / STAGE;
   if (p.stages > 6) p.stages = 6;
   SPC_REQUIRE(p.stages >= 2, "tf32 wgrad: smem budget");
-  const int sms = tc_sm_count();
+  const int sms = sm_count();
   const int groups = p.mgroups * p.n_blocks;
   // split count: as pw_wgrad_kernel's planner, minimise  waves * chunks_per_item * t_chunk + items * elems / atomic_rate
   // (estimates: only their ratio matters).  A tf32 k8 step moves the same bytes and takes the same MMA time as a bf16
@@ -517,11 +454,8 @@ int launch_tf32_wg(const CUtensorMap& tdy, const CUtensorMap& tx, Tf32WgParams p
   p.splits = splits;
   const int smem = p.stages * STAGE + T_SMEM_AUX;
   auto kern = tf32_pw_wgrad_kernel<NBLK, MG>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, T_SMEM_LIMIT));
-    attr_set = true;
-  }
+  const int rc = allow_dynamic_smem((const void*)kern, T_SMEM_LIMIT);
+  if (rc) return rc;
   return run_slices(sl, p.splits, (size_t)p.K * p.C, p.dw, st, [&](int s0, int ns, float* dst, size_t stride) {
     Tf32WgParams q = p;
     q.split0 = s0; q.nsplit = ns; q.dw = dst; q.slice_stride = stride;
@@ -615,8 +549,6 @@ int launch_resample_f32(bool up, const float* src, float* dst, size_t planes, in
   return SPC_OK;
 }
 
-inline bool is_s2(const spc_conv_desc* d) { return d->stride_h == 2 && d->stride_w == 2; }
-
 // repacked weights of op 0 / 1 (wgrad needs none)
 size_t wbytes(const spc_conv_desc* d, int op) {
   if (op == 0) return align1k(wp_bytes(d->K, d->C) + 1024);
@@ -691,6 +623,13 @@ int tf32_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float
     P = (d->H / 2) * (d->W / 2);
   }
   return run_tf32_wgrad(xf, reinterpret_cast<const float*>(dy), dw, d->K, d->C, d->N, P, st, sl);
+}
+
+// Slice copies of tf32_conv_wgrad: as pw_wgrad_kernel's, launch_tf32_wg makes <= 2 * SMs / groups splits of a gradient of
+// <= groups * 128 x 256 floats
+double tf32_wgrad_slice_floats(const spc_conv_desc* d) {
+  const double wn = (double)d->K * d->C * d->R * d->S, sms = sm_count();
+  return 2.0 * sms * (wn < 32768.0 ? wn : 32768.0);
 }
 
 }  // namespace spc

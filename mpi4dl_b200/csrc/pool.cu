@@ -4,8 +4,6 @@
 // exchange + 8 unpack copies) followed by nn.{Max,Avg}Pool2d(padding=0).  Here the window is
 // read straight from the tile and its halo strips (TileView); the padded tensor never exists.
 // These ops are pure HBM streaming (AI ~ 0): one read of x, one write of y.
-#include <cuda.h>
-
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -341,62 +339,27 @@ __global__ void pool3_s1_ring_kernel(const PoolParams p) {
   }
 }
 
-typedef CUresult (*P3EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                               const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                               CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 // x viewed as [planes][H][W]
 template <typename T>
 int launch_pool3_tma(const PoolParams& p, cudaStream_t st) {
   using G = P3Geom<T>;
   SPC_REQUIRE(p.in.x != nullptr && (uintptr_t)p.in.x % 16 == 0 && ((size_t)p.in.W * sizeof(T)) % 16 == 0,
               "pool: TMA needs a 16-byte aligned input and row pitch (W=%d)", p.in.W);
-  static P3EncodeFn enc = nullptr;
-  if (!enc) {
-    void* fp = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fp, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess) {
-      set_error("cuTensorMapEncodeTiled entry point not available");
-      return SPC_ECUDA;
-    }
-    enc = reinterpret_cast<P3EncodeFn>(fp);
-  }
-  // the driver-API encode needs a current context on THIS thread; a backward pass can be the first
-  // CUDA work of an autograd worker thread, which the runtime binds only at its first runtime call
-  // (once per thread: cudaFree is not permitted while the stream is being captured into a CUDA graph)
-  static thread_local bool ctx_bound = false;
-  if (!ctx_bound) {
-    SPC_CHECK_CUDA(cudaFree(nullptr));
-    ctx_bound = true;
-  }
   const size_t planes = (size_t)p.in.N * p.in.C;
   CUtensorMap tm;
-  const cuuint64_t gd[3] = {(cuuint64_t)p.in.W, (cuuint64_t)p.in.H, (cuuint64_t)planes};
-  const cuuint64_t gs[2] = {(cuuint64_t)p.in.W * sizeof(T), (cuuint64_t)p.in.W * p.in.H * sizeof(T)};
-  const cuuint32_t bx[3] = {(cuuint32_t)G::BW, (cuuint32_t)G::BH, 1};
-  const cuuint32_t es[3] = {1, 1, 1};
-  const CUresult r = enc(&tm, sizeof(T) == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3,
-                         const_cast<void*>(p.in.x), gd, gs, bx, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("pool: cuTensorMapEncodeTiled failed (%d) W=%d H=%d planes=%zu", (int)r, p.in.W, p.in.H, planes);
-    return SPC_ECUDA;
-  }
+  const uint64_t dims[3] = {(uint64_t)p.in.W, (uint64_t)p.in.H, (uint64_t)planes};
+  const uint64_t strides[3] = {0, (uint64_t)p.in.W * sizeof(T), (uint64_t)p.in.W * p.in.H * sizeof(T)};
+  const uint32_t box[3] = {(uint32_t)G::BW, (uint32_t)G::BH, 1};
+  int rc = make_tmap(&tm, p.in.x, sizeof(T) == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3,
+                     dims, strides, box, CU_TENSOR_MAP_SWIZZLE_NONE);
+  if (rc) return rc;
   const int tiles_w = (p.in.W + G::TW - 1) / G::TW, tiles_h = (p.in.H + P3_TH - 1) / P3_TH;
   const size_t nt = planes * tiles_w * tiles_h;
   SPC_REQUIRE(nt < (1u << 31), "pool: too many tiles");
   auto kern = pool3_s1_tma_kernel<T>;
-  static bool attr_set = false;   // per instantiation
-  static int sms = 0;
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM_BYTES));
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-    attr_set = true;
-  }
+  rc = allow_dynamic_smem((const void*)kern, G::SMEM_BYTES);
+  if (rc) return rc;
+  const int sms = sm_count();
   const int grid = nt < (size_t)(2 * sms) ? (int)nt : 2 * sms;
   kern<<<grid, P3_THREADS, G::SMEM_BYTES, st>>>(tm, p, tiles_w, tiles_h, (int)nt);
   count_launch();

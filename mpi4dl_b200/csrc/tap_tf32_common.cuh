@@ -1,16 +1,11 @@
 // tap_tf32_common.cuh -- what the TF32 tap kernels of conv_tap_tf32.cu (stride 1) and conv_tap_s2_tf32.cu (stride 2)
-// share: the smem budget, the tf32 rounding of the register operand, the activation tensor maps and the row-segment
-// order of the tiles.
+// share: the smem budget, the activation tensor maps and the row-segment order of the tiles.
 #pragma once
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "wgmma_tf32.cuh"
 
 namespace spc {
-
-int tc_sm_count();
-int make_tmap_f32(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                  const uint32_t* box, bool swizzle);   // gemm_tf32.cu
 
 namespace {
 
@@ -22,22 +17,14 @@ constexpr int TT_SMEM_AUX = 1024 /*align*/ + 512 /*barriers*/;
 constexpr int TT_WRES_MAX = 128 * 1024;       // resident weights at most
 constexpr int TW_MAX_CHAIN = 512;             // wgrad: row segments per item at most (the error bound of the kernels)
 
-inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
-inline size_t align1k(size_t b) { return (b + 1023) & ~(size_t)1023; }
-
-__device__ __forceinline__ uint32_t to_tf32(float v) {   // round to nearest, ties away (the low 13 bits become 0)
-  uint32_t r;
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
-  return r;
-}
-
 // [N][rows][H][W] fp32, box = [1][box_rows][1][box_w px]
 inline int make_act_tmap4(CUtensorMap* m, const void* base, int N, int rows, int H, int W, int box_rows, int box_w,
                           bool swizzle) {
   const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)rows, (uint64_t)N};
   const uint64_t strides[4] = {0, (uint64_t)W * 4, (uint64_t)H * W * 4, (uint64_t)rows * H * W * 4};
   const uint32_t box[4] = {(uint32_t)box_w, 1, (uint32_t)box_rows, 1};
-  return make_tmap_f32(m, base, 4, dims, strides, box, swizzle);
+  return make_tmap(m, base, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, dims, strides, box,
+                   swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE);
 }
 
 // row segment seg of the [N][H][ceil(W / 32)] order -> image, row, first pixel

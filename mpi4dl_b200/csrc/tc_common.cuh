@@ -9,6 +9,16 @@
 #include "wgmma.cuh"
 
 namespace spc {
+
+// host.cu: a tiled tensor map of `rank` <= 5 dims, innermost first; strides_bytes[i] is the stride of dim i >= 1 (entry
+// 0 is unused).  No interleave, 256-byte L2 promotion, out-of-bounds elements read as zero.
+int make_tmap(CUtensorMap* m, const void* base, CUtensorMapDataType type, int rank, const uint64_t* dims,
+              const uint64_t* strides_bytes, const uint32_t* box, CUtensorMapSwizzle swizzle);
+
+// gemm_px.cu: pixel-major 1x1 GEMM (output channels as the wgmma N dimension, NT per tile)
+int run_pw_px(int NT, const CUtensorMap& tw, const CUtensorMap& tx, const CUtensorMap& ty, int M, int Cin, int N, int P,
+              int x5, int y5, const __nv_bfloat16* bias, int sms, cudaStream_t st);
+
 namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -150,6 +160,12 @@ __device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t lbo_b
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
   d |= 1ull << 62;
   return d;
+}
+
+__device__ __forceinline__ uint32_t to_tf32(float v) {   // round to nearest, ties away (the low 13 bits become 0)
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(v));
+  return r;
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {

@@ -30,10 +30,6 @@ namespace spc {
 
 using namespace tc;
 
-int make_tmap_ex(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                 const uint32_t* box, int swizzle128);
-int tc_sm_count();
-
 namespace {
 
 constexpr int WT_THREADS = 640;
@@ -339,18 +335,14 @@ wgrad_tap_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_consta
 
 constexpr int WT_SMEM_LIMIT = 222 * 1024;   // of H100's 227 KB per block
 constexpr int WT_SMEM_AUX = 1024 + 1024;
-inline int rup(int a, int b) { return (a + b - 1) / b * b; }
 
 template <int S, int QC>
 int launch_wt(const CUtensorMap& tp, const CUtensorMap& tq, const WtParams& p, int smem, cudaStream_t st,
               const WgradSlices* sl) {
   auto kern = wgrad_tap_kernel<S, QC>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SPC_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, WT_SMEM_LIMIT));
-    attr_set = true;
-  }
-  const int sms = tc_sm_count();
+  const int rc = allow_dynamic_smem((const void*)kern, WT_SMEM_LIMIT);
+  if (rc) return rc;
+  const int sms = sm_count();
   const int slices = p.N * p.strips * p.row_splits;
   return run_slices(sl, slices, (size_t)p.K * p.C * p.R * p.S, p.dw, st, [&](int s0, int ns, float* dst, size_t stride) {
     WtParams q = p;
@@ -391,7 +383,7 @@ bool wgrad_tap_supported(int K, int C, int R, int S, int H, int W, int stride) {
   if (K > 128 || C > 128) return false;
   // the shapes this kernel serves are those with a plan of 128 / QC taps per pass, the set it was measured on
   // against the shifted-copy path; it runs them in passes of up to 256 / QC taps
-  const int Qc16 = rup(K >= C ? C : K, 16);
+  const int Qc16 = round_up(K >= C ? C : K, 16);
   int rect[MAXPASS][4];
   return plan_passes(R, S, 128 / Qc16, rect) > 0;
 }
@@ -404,9 +396,9 @@ int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, in
   p.ph = (R - 1) / 2; p.pw = (S - 1) / 2;
   p.modeB = K >= C ? 0 : 1;
   p.Pch = p.modeB ? C : K; p.Qch = p.modeB ? K : C;
-  p.Qc16 = rup(p.Qch, 16);
-  p.p_bytes = rup(p.Pch, 8) * 128;
-  p.p_blk = rup(p.p_bytes, 1024);
+  p.Qc16 = round_up(p.Qch, 16);
+  p.p_bytes = round_up(p.Pch, 8) * 128;
+  p.p_blk = round_up(p.p_bytes, 1024);
   p.qt_bytes = p.Qc16 * 128;
   p.raw_bytes = p.Qc16 * RAW_ROW;
   const __nv_bfloat16* P = p.modeB ? x : dy;
@@ -423,22 +415,23 @@ int run_wgrad_tap(const __nv_bfloat16* x, const __nv_bfloat16* dy, float* dw, in
   {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)p.Pch, (uint64_t)N};
     const uint64_t strides[4] = {0, (uint64_t)W * 2, (uint64_t)H * W * 2, (uint64_t)H * W * p.Pch * 2};
-    const uint32_t box[4] = {64, 1, (uint32_t)rup(p.Pch, 8), 1};
-    int rc = make_tmap_ex(&tp, P, 4, dims, strides, box, 1);
+    const uint32_t box[4] = {64, 1, (uint32_t)round_up(p.Pch, 8), 1};
+    int rc = make_tmap(&tp, P, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
   {
     const uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)p.Qch, (uint64_t)N};
     const uint64_t strides[4] = {0, (uint64_t)W * 2, (uint64_t)H * W * 2, (uint64_t)H * W * p.Qch * 2};
     const uint32_t box[4] = {(uint32_t)(S > 1 ? 80 : 64), 1, (uint32_t)p.Qc16, 1};
-    int rc = make_tmap_ex(&tq, Q, 4, dims, strides, box, S > 1 ? 0 : 1);
+    int rc = make_tmap(&tq, Q, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, dims, strides, box,
+                       S > 1 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  const int sms = tc_sm_count();
+  const int sms = sm_count();
   // few channels -> small rows -> wider strips (more bytes per ring slot)
   p.nbw = 1;
   {
-    const int rowb = rup(p.Pch, 8) * 128 + p.Qc16 * 128;
+    const int rowb = round_up(p.Pch, 8) * 128 + p.Qc16 * 128;
     while (p.nbw < 4 && rowb * p.nbw < 12 * 1024 && W % (128 * p.nbw) == 0) p.nbw *= 2;
   }
   p.strips = W / (64 * p.nbw);
