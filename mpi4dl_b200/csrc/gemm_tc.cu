@@ -311,15 +311,24 @@ int launch_shift_copies(const void* x, void* xs, size_t planes, int H, int W, in
 
 // Geometry of one wgmma convolution launch (fprop, or dgrad expressed as a convolution of dY).
 struct TcConv {
-  const __nv_bfloat16* w;      // original filter [K][C][R][S]
+  const __nv_bfloat16* w;      // original filter [K][C][R][S], repacked into wp; null: wp holds the packed weights
+  __nv_bfloat16* wp;           // weights in [taps][Mpad][Cpad] layout (1024-aligned)
   long long sm, sc;            // strides of (output channel m, reduction channel c) in w
   int flip;                    // rotate taps by 180 degrees (dgrad)
   int M, Cin;                  // output channels, reduction channels
   int R, S, ph, pw;            // filter and zero padding
   int H, W, N;                 // input image
   int stride;                  // 1 or 2 (both axes)
-  const __nv_bfloat16* prepacked;   // if set: weights already in [taps][Mpad][Cpad] layout (1024-aligned)
-  int px;                      // 1x1 only: large problems may run on pw_px_gemm_kernel (gemm_px.cu)
+};
+
+// How one op of a bf16 convolution runs (tc_plan picks it)
+enum class TcRoute {
+  None,       // no tensor-core kernel for this op
+  Pw,         // 1x1: pw_gemm_kernel, or pw_px_gemm_kernel (gemm_px.cu) where the plan gives a tile width; pw_wgrad_kernel
+  PwS2,       // 1x1 stride 2: the same kernels on subsampled x (fprop, wgrad), or before a zero-upsample of dx (dgrad)
+  Tap,        // multi-tap without shifted copies: conv_tap_kernel (fprop, dgrad), wgrad_tap_kernel (wgrad)
+  TapGemm,    // multi-tap on pw_gemm_kernel / pw_wgrad_kernel in tap mode, over x or its shifted copies
+  ParityS2,   // dgrad of a 3x3 stride-2 conv: the four parity classes of dx as one 2x2-tap GEMM over dy, then interleave
 };
 
 // Output channels per tile of pw_px_gemm_kernel for a layer with M output channels, or 0 where its tiles would not fit
@@ -335,46 +344,30 @@ int px_tile_channels(int M) {
   return (pad < old_rows && 10 * M >= 9 * pad) ? nt : 0;
 }
 
-// Y[N][M][H*W] = sum_taps Wp[tap][M x Cin] * shift_tap(X[N][Cin][H][W])  (+bias)
-int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bias, __nv_bfloat16* y, void* ws,
-                size_t ws_bytes, cudaStream_t st) {
+// Y[N][M][Ho*Wo] = sum_taps Wp[tap][M x Cin] * shift_tap(X[N][Cin][H][W])  (+bias) on conv_tap_kernel (route Tap),
+// pw_px_gemm_kernel (1x1, nt > 0) or pw_gemm_kernel; xs: where the column-shifted copies of X go, null for none
+int run_conv_tc(const TcConv& c, TcRoute route, int nt, __nv_bfloat16* xs, const __nv_bfloat16* x,
+                const __nv_bfloat16* bias, __nv_bfloat16* y, cudaStream_t st) {
   const int taps = c.R * c.S;
   const int cs = c.stride;
   const int Ho = c.H / cs, Wo = c.W / cs;
   const int Pin = c.H * c.W, P = Ho * Wo;            // P: output pixels per image
-  // pixel-major kernel: 1x1 layers whose output channels it tiles better, with at least two 128-pixel tiles per SM
-  // (below that the persistent CTAs get one tile each and pw_gemm_kernel's 128-row blocks cost no more)
-  const int nt = (c.px && taps == 1) ? px_tile_channels(c.M) : 0;
-  const bool px = nt && (long long)c.N * ((P + BN - 1) / BN) >= 2ll * sm_count();
-  const int Mpad = round_up(c.M, px ? nt : 128), Cpad = round_up(c.Cin, BK);
-  const bool v2 = taps > 1 && tap_v2_supported(c.M, c.Cin, c.R, c.S, c.H, c.W, c.N, cs);
-  const bool copies = (c.S > 1 || cs > 1) && taps > 1 && !v2;   // column-shifted (and subsampled) copies of the input
-  const uintptr_t ws0 = reinterpret_cast<uintptr_t>(ws);
-  const uintptr_t wp_addr = (ws0 + 1023) & ~(uintptr_t)1023;
-  const size_t wp_bytes = c.prepacked ? 0 : (size_t)taps * Mpad * Cpad * 2;
-  const uintptr_t xs_addr = (wp_addr + wp_bytes + 1023) & ~(uintptr_t)1023;
-  const size_t xs_bytes = copies ? (size_t)c.S * c.N * c.Cin * c.H * Wo * 2 : 0;
-  const size_t need = (xs_addr - ws0) + xs_bytes;
-  SPC_REQUIRE((ws && ws_bytes >= need) || need <= 1024, "wgmma conv: workspace too small (%zu < %zu)", ws_bytes, need);
-  const __nv_bfloat16* wp = c.prepacked;
-  if (!c.prepacked) {
-    __nv_bfloat16* wpm = reinterpret_cast<__nv_bfloat16*>(wp_addr);
+  const int rows = nt ? nt : 128;                    // output channels per weight box and output tile
+  const int Mpad = round_up(c.M, rows), Cpad = round_up(c.Cin, BK);
+  if (c.w) {
     const int total = taps * Mpad * Cpad;
     int blocks = (total + 255) / 256;
     if (blocks > 1184) blocks = 1184;
-    repack_weights_kernel<<<blocks, 256, 0, st>>>(c.w, wpm, c.M, c.Cin, Mpad, Cpad, taps, c.sm, c.sc, c.flip);
+    repack_weights_kernel<<<blocks, 256, 0, st>>>(c.w, c.wp, c.M, c.Cin, Mpad, Cpad, taps, c.sm, c.sc, c.flip);
     count_launch();
     SPC_CHECK_CUDA(cudaGetLastError());
-    wp = wpm;
   }
-  if (v2)
-    return run_conv_tap_v2(wp, Mpad, Cpad, x, bias, y, c.M, c.Cin, c.R, c.S, c.ph, c.H, c.W, c.N, st);
-  const __nv_bfloat16* xsrc = x;
-  if (copies) {
-    void* xs = reinterpret_cast<void*>(xs_addr);
+  if (route == TcRoute::Tap)
+    return run_conv_tap_v2(c.wp, Mpad, Cpad, x, bias, y, c.M, c.Cin, c.R, c.S, c.ph, c.H, c.W, c.N, st);
+  if (xs) {
     int rc0 = launch_shift_copies(x, xs, (size_t)c.N * c.Cin, c.H, c.W, c.S, c.pw, cs, st);
     if (rc0) return rc0;
-    xsrc = reinterpret_cast<const __nv_bfloat16*>(xs);
+    x = xs;
   }
   CUtensorMap tw, tx, tx4, ty;
   // 5-d boxes (see PwParams::x5) for the layers whose channel planes span several 2 MB pages (from 4 MB planes)
@@ -384,24 +377,17 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
   {
     const uint64_t dims[2] = {(uint64_t)Cpad, (uint64_t)taps * Mpad};
     const uint64_t strides[2] = {0, (uint64_t)Cpad * 2};
-    const uint32_t box[2] = {BK, px ? (uint32_t)nt : 128u};
-    int rc = make_tmap(&tw, wp, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+    const uint32_t box[2] = {BK, (uint32_t)rows};
+    int rc = make_tmap(&tw, c.wp, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
   int rc;
-  if (px) {
-    rc = x5 ? make_act_tmap5(&tx, x, Pin, c.Cin, c.N, BK / 8, BN / 64) : make_act_tmap(&tx, x, Pin, c.Cin, c.N, BK);
-    if (rc) return rc;
-    rc = y5 ? make_act_tmap5(&ty, y, P, c.M, c.N, nt / 8, 2) : make_act_tmap(&ty, y, P, c.M, c.N, nt);
-    if (rc) return rc;
-    return run_pw_px(nt, tw, tx, ty, c.M, c.Cin, c.N, P, x5, y5, bias, sm_count(), st);
-  }
   if (taps > 1) {
     // (copies of) the input as [img][Cin][H][Wo]; img = n + s*N for the copy of filter column s
-    const uint64_t dims[4] = {(uint64_t)Wo, (uint64_t)c.H, (uint64_t)c.Cin, (uint64_t)c.N * (copies ? c.S : 1)};
+    const uint64_t dims[4] = {(uint64_t)Wo, (uint64_t)c.H, (uint64_t)c.Cin, (uint64_t)c.N * (xs ? c.S : 1)};
     const uint64_t strides[4] = {0, (uint64_t)Wo * 2, (uint64_t)c.H * Wo * 2, (uint64_t)c.H * Wo * c.Cin * 2};
     const uint32_t box[4] = {64, 1, BK, 1};
-    rc = make_tmap(&tx4, xsrc, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+    rc = make_tmap(&tx4, x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
     tx = tx4;
   } else {
@@ -409,13 +395,14 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
     if (rc) return rc;
     tx4 = tx;
   }
-  rc = y5 ? make_act_tmap5(&ty, y, P, c.M, c.N, 16, 2) : make_act_tmap(&ty, y, P, c.M, c.N, 128);
+  rc = y5 ? make_act_tmap5(&ty, y, P, c.M, c.N, rows / 8, 2) : make_act_tmap(&ty, y, P, c.M, c.N, rows);
   if (rc) return rc;
+  if (nt) return run_pw_px(nt, tw, tx, ty, c.M, c.Cin, c.N, P, x5, y5, bias, sm_count(), st);
   PwParams p{};
   p.x5 = x5; p.y5 = y5;
   p.bias = bias; p.M = c.M; p.Cin = c.Cin; p.P = P; p.N = c.N;
   p.taps = taps; p.S = c.S; p.ph = c.ph; p.pw = c.pw; p.W = Wo; p.Mpad = Mpad;
-  p.shiftN = copies ? c.N : 0;
+  p.shiftN = xs ? c.N : 0;
   p.rowmul = cs;
   // groups of at most two 128-row blocks of output channels: a consumer thread holds 64 fp32 accumulators per block
   const int MBtot = Mpad / 128;
@@ -424,18 +411,6 @@ int run_conv_tc(const TcConv& c, const __nv_bfloat16* x, const __nv_bfloat16* bi
   p.tiles_per_image = (P + BN - 1) / BN;
   p.num_tiles = p.tiles_per_image * c.N * p.num_mg;
   return mb == 2 ? launch_pw<2>(tw, tx, tx4, ty, p, st) : launch_pw<1>(tw, tx, tx4, ty, p, st);
-}
-
-// pointwise helper (1x1): Y[N][M][P] = Wp[M x Cin] * X[N][Cin][P]; px = 0 keeps it on pw_gemm_kernel
-int run_pw(const __nv_bfloat16* w, int ld, int transpose, int M, int Cin, const __nv_bfloat16* x,
-           const __nv_bfloat16* bias, __nv_bfloat16* y, int N, int P, void* ws, size_t ws_bytes, cudaStream_t st,
-           int px = 1) {
-  TcConv c{};
-  c.px = px;
-  c.w = w;
-  c.sm = transpose ? 1 : ld; c.sc = transpose ? ld : 1; c.flip = 0;
-  c.M = M; c.Cin = Cin; c.R = 1; c.S = 1; c.ph = 0; c.pw = 0; c.H = 1; c.W = P; c.N = N; c.stride = 1;
-  return run_conv_tc(c, x, bias, y, ws, ws_bytes, st);
 }
 
 // ---- wgrad kernel: dW[K x C x taps] += dY[K x P] * shift_tap(X)[C x P]^T -------------------------
@@ -1001,7 +976,6 @@ int launch_shift_copies(const void* x, void* xs, size_t planes, int H, int W, in
 }
 
 bool tap_shape_ok(const spc_conv_desc* d) {   // odd RxS "same" convs, stride 1 or 2, on 64-pixel output row segments
-  if (d->dtype != SPC_BF16) return false;
   if (d->R * d->S == 1 || d->R * d->S > 49) return false;
   if ((d->R & 1) == 0 || (d->S & 1) == 0) return false;
   const bool s1 = d->stride_h == 1 && d->stride_w == 1, s2 = d->stride_h == 2 && d->stride_w == 2;
@@ -1013,7 +987,6 @@ bool tap_shape_ok(const spc_conv_desc* d) {   // odd RxS "same" convs, stride 1 
 }
 
 bool pw_shape_ok(const spc_conv_desc* d) {
-  if (d->dtype != SPC_BF16) return false;
   if (d->R != 1 || d->S != 1) return false;
   long long P = (long long)d->H * d->W;
   if (is_s2(d)) {
@@ -1026,99 +999,132 @@ bool pw_shape_ok(const spc_conv_desc* d) {
   return true;
 }
 
+// Op 0 / 1 / 2 (fprop, dgrad, wgrad) of a bf16 convolution: its route, and where its buffers go in the workspace.
+// tc_plan is the one place these are decided.
+struct TcRegion {
+  size_t off, bytes;   // from the workspace's first 1 KB boundary
+};
+struct TcPlan {
+  TcRoute route;
+  bool copies;         // the GEMM reads S column-shifted (stride 2: and subsampled) copies of its input, made in xs
+  int nt;              // Pw / PwS2 fprop and dgrad: pw_px_gemm_kernel's tile width; 0: pw_gemm_kernel
+  TcRegion wp;         // repacked weights (ParityS2: of the 2x2-tap GEMM)
+  TcRegion xs;         // the shifted copies (ParityS2: of dy); PwS2: the subsampled x, or dgrad's W^T dy
+  TcRegion tmp;        // ParityS2: the four parity-class planes of dx before the interleave
+  size_t total;        // what spc_conv_workspace_bytes asks for: the regions plus slack for the alignment
+};
+
+TcPlan tc_plan(const spc_conv_desc* d, int op) {
+  TcPlan pl{};
+  const bool s2 = is_s2(d);
+  const size_t taps = (size_t)d->R * d->S, N = d->N;
+  const int cs = d->stride_w, Ho = d->H / cs, Wo = d->W / cs;
+  // the GEMM: M output channels over Cin reduction channels (dgrad: the transposed filter over dy)
+  const int M = op == 1 ? d->C : d->K, Cin = op == 1 ? d->K : d->C;
+  if (d->dtype != SPC_BF16) return pl;
+  if (pw_shape_ok(d)) {
+    pl.route = s2 ? TcRoute::PwS2 : TcRoute::Pw;
+    if (s2) pl.xs.bytes = N * d->C * Ho * Wo * 2;
+    // pixel-major kernel: 1x1 layers whose output channels it tiles better, with at least two 128-pixel tiles per SM
+    // (below that the persistent CTAs get one tile each and pw_gemm_kernel's 128-row blocks cost no more)
+    const int nt = op == 2 ? 0 : px_tile_channels(M);
+    if (nt && (long long)d->N * ((Ho * Wo + BN - 1) / BN) >= 2ll * sm_count()) pl.nt = nt;
+  } else if (!tap_shape_ok(d)) {
+    return pl;
+  } else if (op == 1 && s2) {
+    if (d->R != 3 || d->S != 3 || 4 * d->C > 2048) return pl;
+    pl.route = TcRoute::ParityS2;
+    pl.wp.bytes = 4ull * round_up(4 * d->C, 128) * round_up(d->K, BK) * 2;
+    pl.xs.bytes = 2ull * N * d->K * Ho * Wo * 2;
+    pl.tmp.bytes = 4ull * N * d->C * Ho * Wo * 2;
+    pl.total = align1k(pl.wp.bytes) + align1k(pl.xs.bytes) + align1k(pl.tmp.bytes) + 8192;
+  } else if (op == 2 ? wgrad_tap_supported(d->K, d->C, d->R, d->S, d->H, d->W, cs)
+                     : tap_v2_supported(M, Cin, d->R, d->S, d->H, d->W, d->N, cs)) {
+    pl.route = TcRoute::Tap;   // conv_tap.cu / wgrad_tap.cu form the horizontal taps in shared memory: no copies
+  } else {
+    pl.route = TcRoute::TapGemm;
+    pl.copies = d->S > 1 || cs > 1;
+    if (pl.copies) pl.xs.bytes = (size_t)d->S * N * Cin * d->H * Wo * 2;
+  }
+  if (pl.route != TcRoute::ParityS2) {
+    // The total counts the weights at 128-row padding whatever nt is.  Where nt pads them further (M = 375..384,
+    // 1124..1152, ...), the regions can outgrow it and tc_regions turns the call down.
+    if (op != 2) pl.wp.bytes = taps * round_up(M, pl.nt ? pl.nt : 128) * round_up(Cin, BK) * 2;
+    pl.total = (op == 2 ? 0 : taps * round_up(M, 128) * round_up(Cin, BK) * 2 + 1024) + 4096;
+    if (pl.route == TcRoute::PwS2 || pl.copies) pl.total += align1k(pl.xs.bytes) + (pl.copies ? 2048 : 1024);
+  }
+  pl.xs.off = align1k(pl.wp.bytes);
+  pl.tmp.off = align1k(pl.xs.off + pl.xs.bytes);
+  return pl;
+}
+
+// The start of pl's regions in ws, once they are known to fit its ws_bytes
+int tc_regions(const TcPlan& pl, void* ws, size_t ws_bytes, uint8_t** base) {
+  const uintptr_t b = align1k(reinterpret_cast<uintptr_t>(ws));
+  const size_t end = pl.tmp.off + pl.tmp.bytes, fit = b - reinterpret_cast<uintptr_t>(ws) + end;
+  const size_t need = fit > pl.total ? fit : pl.total;
+  SPC_REQUIRE(!end || (ws && ws_bytes >= need), "wgmma conv: workspace too small (%zu < %zu)", ws_bytes, need);
+  *base = reinterpret_cast<uint8_t*>(b);
+  return SPC_OK;
+}
+
 }  // namespace
 
 bool tc_supported(const spc_conv_desc* d, int op) {
-  if (pw_shape_ok(d)) return true;
-  if (tap_shape_ok(d)) {
-    if (tc_workspace_bytes(d, op) > (24ull << 30)) return false;   // shifted copies would not fit comfortably
-    if (op == 1 && is_s2(d)) return d->R == 3 && d->S == 3 && 4 * d->C <= 2048;   // parity-class dgrad
-    return true;
-  }
-  return false;
+  const TcPlan pl = tc_plan(d, op);
+  if (pl.route == TcRoute::Pw || pl.route == TcRoute::PwS2) return true;
+  return pl.route != TcRoute::None && pl.total <= (24ull << 30);   // shifted copies would not fit comfortably
 }
 
-// workspace = [repacked weights | subsampled activations (stride-2 only)]
-static size_t wbytes(const spc_conv_desc* d, int op) {
-  const size_t taps = (size_t)d->R * d->S;
-  if (op == 0) return align1k(taps * round_up(d->K, 128) * round_up(d->C, BK) * 2 + 1024);
-  if (op == 1) return align1k(taps * round_up(d->C, 128) * round_up(d->K, BK) * 2 + 1024);
-  return 0;
-}
-size_t tc_workspace_bytes(const spc_conv_desc* d, int op) {
-  const size_t taps = (size_t)d->R * d->S;
-  const int cs = d->stride_w;
-  size_t b = wbytes(d, op) + 4096;
-  if (taps == 1) {
-    if (is_s2(d)) b += align1k((size_t)d->N * d->C * (d->H / 2) * (d->W / 2) * 2) + 1024;
-    return b;
-  }
-  const size_t Ho = d->H / cs, Wo = d->W / cs;
-  if (op == 1 && is_s2(d)) {
-    // Wq[4][4C pad][K pad] + 2 column-shifted copies of dy + the 4-class output planes
-    b = align1k(4ull * round_up(4 * d->C, 128) * round_up(d->K, BK) * 2) + 4096;
-    b += align1k(2ull * d->N * d->K * Ho * Wo * 2) + align1k(4ull * d->N * d->C * Ho * Wo * 2) + 4096;
-    return b;
-  }
-  if (op != 2 && tap_v2_supported(op == 1 ? d->C : d->K, op == 1 ? d->K : d->C, d->R, d->S, d->H, d->W, d->N, cs))
-    return b;               // conv_tap.cu forms the horizontal taps in shared memory: no copies
-  if (op == 2 && wgrad_tap_supported(d->K, d->C, d->R, d->S, d->H, d->W, cs))
-    return b;               // wgrad_tap.cu likewise
-  if (d->S > 1 || cs > 1)   // S column-shifted (stride 2: also subsampled) copies of the conv input
-    b += align1k((size_t)d->S * d->N * (op == 1 ? d->K : d->C) * d->H * Wo * 2) + 2048;
-  return b;
-}
+size_t tc_workspace_bytes(const spc_conv_desc* d, int op) { return tc_plan(d, op).total; }
 
 int tc_conv_fwd(const spc_conv_desc* d, const void* x, const void* w, const void* bias, void* y, void* ws,
                 size_t ws_bytes, cudaStream_t st) {
-  SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 0), "wgmma conv: workspace too small");
-  if (d->R * d->S > 1) {
-    TcConv c{};
-    c.w = reinterpret_cast<const __nv_bfloat16*>(w);
-    c.sm = (long long)d->C * d->R * d->S; c.sc = (long long)d->R * d->S; c.flip = 0;
-    c.M = d->K; c.Cin = d->C; c.R = d->R; c.S = d->S; c.ph = d->pad_h; c.pw = d->pad_w;
-    c.H = d->H; c.W = d->W; c.N = d->N; c.stride = d->stride_h;
-    return run_conv_tc(c, reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(bias),
-                       reinterpret_cast<__nv_bfloat16*>(y), ws, ws_bytes, st);
-  }
-  if (is_s2(d)) {   // Y = W * subsample(X)
-    void* xs = reinterpret_cast<void*>(align1k(reinterpret_cast<uintptr_t>(ws) + wbytes(d, 0)));
-    int rc = launch_resample(false, x, xs, (size_t)d->N * d->C, d->H, d->W, st);
+  const TcPlan pl = tc_plan(d, 0);
+  uint8_t* base;
+  int rc = tc_regions(pl, ws, ws_bytes, &base);
+  if (rc) return rc;
+  __nv_bfloat16* xs = reinterpret_cast<__nv_bfloat16*>(base + pl.xs.off);
+  TcConv c{};
+  c.w = reinterpret_cast<const __nv_bfloat16*>(w);
+  c.wp = reinterpret_cast<__nv_bfloat16*>(base + pl.wp.off);
+  c.sm = (long long)d->C * d->R * d->S; c.sc = (long long)d->R * d->S; c.flip = 0;
+  c.M = d->K; c.Cin = d->C; c.R = d->R; c.S = d->S; c.ph = d->pad_h; c.pw = d->pad_w;
+  c.H = d->H; c.W = d->W; c.N = d->N; c.stride = d->stride_h;
+  if (pl.route == TcRoute::PwS2) {   // Y = W * subsample(X)
+    rc = launch_resample(false, x, xs, (size_t)d->N * d->C, d->H, d->W, st);
     if (rc) return rc;
-    return run_pw(reinterpret_cast<const __nv_bfloat16*>(w), d->C, 0, d->K, d->C,
-                  reinterpret_cast<const __nv_bfloat16*>(xs), reinterpret_cast<const __nv_bfloat16*>(bias),
-                  reinterpret_cast<__nv_bfloat16*>(y), d->N, (d->H / 2) * (d->W / 2), ws, wbytes(d, 0), st);
+    x = xs; c.H /= 2; c.W /= 2; c.stride = 1;
   }
-  return run_pw(reinterpret_cast<const __nv_bfloat16*>(w), d->C, 0, d->K, d->C,
-                reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(bias),
-                reinterpret_cast<__nv_bfloat16*>(y), d->N, d->H * d->W, ws, ws_bytes, st);
+  return run_conv_tc(c, pl.route, pl.nt, pl.copies ? xs : nullptr, reinterpret_cast<const __nv_bfloat16*>(x),
+                     reinterpret_cast<const __nv_bfloat16*>(bias), reinterpret_cast<__nv_bfloat16*>(y), st);
 }
 
 int tc_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* dx, void* ws, size_t ws_bytes,
                   cudaStream_t st) {
   // dX[C x P] = W^T[C x K] * dY[K x P]
-  SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 1), "wgmma conv: workspace too small");
-  if (d->R * d->S > 1 && is_s2(d)) {   // 3x3 stride 2: four parity classes as channel groups, then interleave
+  const TcPlan pl = tc_plan(d, 1);
+  uint8_t* base;
+  int rc = tc_regions(pl, ws, ws_bytes, &base);
+  if (rc) return rc;
+  const __nv_bfloat16* dyb = reinterpret_cast<const __nv_bfloat16*>(dy);
+  __nv_bfloat16* xs = reinterpret_cast<__nv_bfloat16*>(base + pl.xs.off);
+  TcConv c{};
+  c.wp = reinterpret_cast<__nv_bfloat16*>(base + pl.wp.off);
+  if (pl.route == TcRoute::ParityS2) {   // four parity classes as channel groups, then interleave
     const int Ho = d->H / 2, Wo = d->W / 2;
     const int Mq = 4 * d->C, Mpad = round_up(Mq, 128), Kpad = round_up(d->K, BK);
-    uintptr_t a = align1k(reinterpret_cast<uintptr_t>(ws));
-    __nv_bfloat16* wq = reinterpret_cast<__nv_bfloat16*>(a);
-    a = align1k(a + (size_t)4 * Mpad * Kpad * 2);
-    __nv_bfloat16* tmp = reinterpret_cast<__nv_bfloat16*>(a);
-    a = align1k(a + (size_t)4 * d->N * d->C * Ho * Wo * 2);
+    __nv_bfloat16* tmp = reinterpret_cast<__nv_bfloat16*>(base + pl.tmp.off);
     {
       const int total = 4 * Mpad * Kpad;
       int blocks = (total + 255) / 256;
       if (blocks > 1184) blocks = 1184;
-      repack_dgrad_s2_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(w), wq, d->K, d->C, Mpad, Kpad);
+      repack_dgrad_s2_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const __nv_bfloat16*>(w), c.wp, d->K, d->C, Mpad, Kpad);
       count_launch();
       SPC_CHECK_CUDA(cudaGetLastError());
     }
-    TcConv c{};
-    c.prepacked = wq;
     c.M = Mq; c.Cin = d->K; c.R = 2; c.S = 2; c.ph = 0; c.pw = 0; c.H = Ho; c.W = Wo; c.N = d->N; c.stride = 1;
-    int rc = run_conv_tc(c, reinterpret_cast<const __nv_bfloat16*>(dy), nullptr, tmp, reinterpret_cast<void*>(a),
-                         ws_bytes - (a - reinterpret_cast<uintptr_t>(ws)), st);
+    rc = run_conv_tc(c, TcRoute::TapGemm, 0, xs, dyb, nullptr, tmp, st);
     if (rc) return rc;
     const size_t total = (size_t)d->N * d->C * 2 * Ho * (Wo / 8);
     size_t blocks = (total + 255) / 256;
@@ -1128,56 +1134,43 @@ int tc_conv_dgrad(const spc_conv_desc* d, const void* dy, const void* w, void* d
     SPC_CHECK_CUDA(cudaGetLastError());
     return SPC_OK;
   }
-  if (d->R * d->S > 1) {   // stride-1 dgrad = correlation of dY with the transposed, 180-degree rotated filter
-    TcConv c{};
-    c.w = reinterpret_cast<const __nv_bfloat16*>(w);
-    c.sm = (long long)d->R * d->S; c.sc = (long long)d->C * d->R * d->S; c.flip = 1;
-    c.M = d->C; c.Cin = d->K; c.R = d->R; c.S = d->S; c.ph = d->R - 1 - d->pad_h; c.pw = d->S - 1 - d->pad_w;
-    c.H = d->H; c.W = d->W; c.N = d->N; c.stride = 1;
-    return run_conv_tc(c, reinterpret_cast<const __nv_bfloat16*>(dy), nullptr, reinterpret_cast<__nv_bfloat16*>(dx), ws,
-                       ws_bytes, st);
-  }
-  if (is_s2(d)) {   // dX = zero_upsample(W^T * dY)
-    void* gs = reinterpret_cast<void*>(align1k(reinterpret_cast<uintptr_t>(ws) + wbytes(d, 1)));
-    int rc = run_pw(reinterpret_cast<const __nv_bfloat16*>(w), d->C, 1, d->C, d->K,
-                    reinterpret_cast<const __nv_bfloat16*>(dy), nullptr, reinterpret_cast<__nv_bfloat16*>(gs), d->N,
-                    (d->H / 2) * (d->W / 2), ws, wbytes(d, 1), st);
+  // correlation of dY with the transposed, 180-degree rotated filter
+  c.w = reinterpret_cast<const __nv_bfloat16*>(w);
+  c.sm = (long long)d->R * d->S; c.sc = (long long)d->C * d->R * d->S; c.flip = 1;
+  c.M = d->C; c.Cin = d->K; c.R = d->R; c.S = d->S; c.ph = d->R - 1 - d->pad_h; c.pw = d->S - 1 - d->pad_w;
+  c.H = d->H; c.W = d->W; c.N = d->N; c.stride = 1;
+  if (pl.route == TcRoute::PwS2) {   // dX = zero_upsample(W^T * dY)
+    c.H /= 2; c.W /= 2;
+    rc = run_conv_tc(c, pl.route, pl.nt, nullptr, dyb, nullptr, xs, st);
     if (rc) return rc;
-    return launch_resample(true, gs, dx, (size_t)d->N * d->C, d->H, d->W, st);
+    return launch_resample(true, xs, dx, (size_t)d->N * d->C, d->H, d->W, st);
   }
-  return run_pw(reinterpret_cast<const __nv_bfloat16*>(w), d->C, 1, d->C, d->K,
-                reinterpret_cast<const __nv_bfloat16*>(dy), nullptr, reinterpret_cast<__nv_bfloat16*>(dx), d->N,
-                d->H * d->W, ws, ws_bytes, st);
+  return run_conv_tc(c, pl.route, pl.nt, pl.copies ? xs : nullptr, dyb, nullptr, reinterpret_cast<__nv_bfloat16*>(dx),
+                     st);
 }
 
 int tc_conv_wgrad(const spc_conv_desc* d, const void* x, const void* dy, float* dw, void* ws, size_t ws_bytes,
                   cudaStream_t st, const WgradSlices* sl) {
   // the kernels accumulate into dw with atomics; api.cu has zeroed it unless the caller accumulates
+  const TcPlan pl = tc_plan(d, 2);
+  uint8_t* base;
+  int rc = tc_regions(pl, ws, ws_bytes, &base);
+  if (rc) return rc;
   const __nv_bfloat16* xb = reinterpret_cast<const __nv_bfloat16*>(x);
   const __nv_bfloat16* dyb = reinterpret_cast<const __nv_bfloat16*>(dy);
-  if (d->R * d->S > 1) {
-    const int cs = d->stride_h;
-    if (wgrad_tap_supported(d->K, d->C, d->R, d->S, d->H, d->W, cs))
-      return run_wgrad_tap(xb, dyb, dw, d->K, d->C, d->N, d->H, d->W, d->R, d->S, st, sl);
-    const bool copies = d->S > 1 || cs > 1;
-    if (copies) {
-      SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 2), "wgmma wgrad: workspace too small");
-      void* xs = reinterpret_cast<void*>(align1k(reinterpret_cast<uintptr_t>(ws)));
-      int rc = launch_shift_copies(x, xs, (size_t)d->N * d->C, d->H, d->W, d->S, d->pad_w, cs, st);
-      if (rc) return rc;
-      xb = reinterpret_cast<const __nv_bfloat16*>(xs);
-    }
-    return run_wgrad(xb, dyb, dw, d->K, d->C, d->N, d->H / cs, d->W / cs, d->H, d->R, d->S, d->pad_h, cs, copies, st, sl);
-  }
-  if (is_s2(d)) {
-    SPC_REQUIRE(ws && ws_bytes >= tc_workspace_bytes(d, 2), "wgmma wgrad: workspace too small");
-    void* xs = reinterpret_cast<void*>(align1k(reinterpret_cast<uintptr_t>(ws)));
-    int rc = launch_resample(false, x, xs, (size_t)d->N * d->C, d->H, d->W, st);
+  __nv_bfloat16* xs = reinterpret_cast<__nv_bfloat16*>(base + pl.xs.off);
+  if (pl.route == TcRoute::Tap) return run_wgrad_tap(xb, dyb, dw, d->K, d->C, d->N, d->H, d->W, d->R, d->S, st, sl);
+  int H = d->H, W = d->W, cs = d->stride_h;
+  if (pl.route == TcRoute::PwS2) {   // dW = dY * subsample(X)^T
+    rc = launch_resample(false, x, xs, (size_t)d->N * d->C, d->H, d->W, st);
     if (rc) return rc;
-    return run_wgrad(reinterpret_cast<const __nv_bfloat16*>(xs), dyb, dw, d->K, d->C, d->N, 1, (d->H / 2) * (d->W / 2), 1,
-                     1, 1, 0, 1, false, st, sl);
+    xb = xs; H /= 2; W /= 2; cs = 1;
+  } else if (pl.copies) {
+    rc = launch_shift_copies(x, xs, (size_t)d->N * d->C, d->H, d->W, d->S, d->pad_w, cs, st);
+    if (rc) return rc;
+    xb = xs;
   }
-  return run_wgrad(xb, dyb, dw, d->K, d->C, d->N, 1, d->H * d->W, 1, 1, 1, 0, 1, false, st, sl);
+  return run_wgrad(xb, dyb, dw, d->K, d->C, d->N, H / cs, W / cs, H, d->R, d->S, d->pad_h, cs, pl.copies, st, sl);
 }
 
 // Slice copies of tc_conv_wgrad: pw_wgrad_kernel (launch_wg) makes <= 2 * SMs / groups splits of a gradient of <= groups
@@ -1196,9 +1189,14 @@ double tc_wgrad_slice_floats(const spc_conv_desc* d) {
 size_t tc_pw_workspace_bytes(int M, int Cin) { return (size_t)round_up(M, 128) * round_up(Cin, BK) * 2 + 4096; }
 int tc_pw_fwd(const void* w, int ld, int M, int Cin, const void* x, const void* bias, void* y, int P, void* ws, size_t ws_bytes,
               cudaStream_t st) {
-  return run_pw(reinterpret_cast<const __nv_bfloat16*>(w), ld, 0, M, Cin, reinterpret_cast<const __nv_bfloat16*>(x),
-                reinterpret_cast<const __nv_bfloat16*>(bias), reinterpret_cast<__nv_bfloat16*>(y), 1, P, ws, ws_bytes, st,
-                0);
+  SPC_REQUIRE(ws && ws_bytes >= tc_pw_workspace_bytes(M, Cin), "wgmma conv: workspace too small");
+  TcConv c{};
+  c.w = reinterpret_cast<const __nv_bfloat16*>(w);
+  c.wp = reinterpret_cast<__nv_bfloat16*>(align1k(reinterpret_cast<uintptr_t>(ws)));
+  c.sm = ld; c.sc = 1; c.flip = 0;
+  c.M = M; c.Cin = Cin; c.R = 1; c.S = 1; c.ph = 0; c.pw = 0; c.H = 1; c.W = P; c.N = 1; c.stride = 1;
+  return run_conv_tc(c, TcRoute::Pw, 0, nullptr, reinterpret_cast<const __nv_bfloat16*>(x),
+                     reinterpret_cast<const __nv_bfloat16*>(bias), reinterpret_cast<__nv_bfloat16*>(y), st);
 }
 int tc_pw_wgrad(const void* x, const void* dy, float* dw, int K, int C, int P, cudaStream_t st, const WgradSlices* sl) {
   return run_wgrad(reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<const __nv_bfloat16*>(dy), dw, K, C, 1, 1, P, 1, 1, 1,
